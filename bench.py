@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- the adjoint hot path on B200: dRdW^T*psi throughput (GCells/s) and adjoint-solve wall time.
+"""bench.py -- the adjoint hot path on H100: dRdW^T*psi throughput (GCells/s) and adjoint-solve wall time.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--cells C] [--scaling weak|strong]
+                  [--dump-outputs DIR]
 
 A "step" is one matrix-free product y = diag(n) (dR/dW)^T psi over the whole mesh (the body of the reference's GMRES
 shell-matrix callback, DASolver.C:1364-1409).  Workload: BASELINE.json configs[1], "DASimpleFoam NACA0012 SA turbulence
@@ -9,7 +10,8 @@ shell-matrix callback, DASolver.C:1364-1409).  Workload: BASELINE.json configs[1
 (16x12 tiles, the order a bandwidth-reducing renumbering leaves), analytic boundary-layer state + 0.1 % seeded noise.
 With N GPUs: weak scaling (default; N x cells, RCB partitions) or strong scaling (--scaling strong; the same mesh).
 The adjoint solve (preconditioner assembly + Krylov solve of [dRdW]^T psi = dFdW) runs at every N.
-One JSON line on stdout (rank 0).
+One JSON line on stdout (rank 0).  --dump-outputs DIR also writes what the timed path returned in its last step as
+DIR/<name>.npy (see dump_outputs), so that two builds can be compared output for output on the same seeded inputs.
 """
 import argparse
 import json
@@ -223,8 +225,6 @@ def run_reference(args, rank):
         last = arm.run(reps)
         if i >= args.warmup:
             vals.append(last["value"])
-        if i >= args.warmup + 2:  # bounded: three timed samples
-            break
     arm.close()
     v = float(np.mean(vals))
     last["value"] = v
@@ -272,6 +272,39 @@ def global_state(mesh, comp, U0c, thermo):
     return Wg
 
 
+DUMP_SAMPLE = 1 << 20  # values kept per array (8 MB in float64); a longer array is sampled at fixed, seeded indices
+
+
+def dump_outputs(d, arrays, rank, world):
+    """Write each array as d/<name>.npy in float64.  An array longer than DUMP_SAMPLE / world is replaced by its values at the
+    sorted indices np.random.default_rng(0).choice(len, k, replace=False), which are written beside it as <name>_index.npy
+    (float64, exact below 2**53): at most three arrays of 16 MB with their indices, 48 MB in all.  Several GPUs: every rank
+    writes its own local arrays, with the suffix _rank<r>."""
+    os.makedirs(d, exist_ok=True)
+    k = DUMP_SAMPLE // world
+    sfx = "_rank%d" % rank if world > 1 else ""
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float64).ravel()
+        if a.size > k:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, k, replace=False))
+            np.save(os.path.join(d, name + "_index" + sfx + ".npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(d, name + sfx + ".npy"), a)
+
+
+def device_info(local_rank):
+    """The card's name and power limit: an absolute rate is only meaningful beside them."""
+    import torch
+    info = {"name": torch.cuda.get_device_name(local_rank), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(local_rank)],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        info["power_limit_w"] = float(out.splitlines()[0])
+    except Exception:
+        pass
+    return info
+
+
 def main():
     global _REAL_STDOUT
     sys.stdout.flush()
@@ -308,7 +341,12 @@ def main():
                          "(the RevB<6,7> / FwdB<6,7> kernel variants instead of the light <6,0> ones); not the default workload")
     ap.add_argument("--primal-iters", type=int, default=None,
                     help="run that many SIMPLE iterations (solvePrimal on the GPU) from the synthetic state before the adjoint legs (1 GPU)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the product dRdW^T psi of the last timed step, the adjoint solution and (with "
+                         "--primal-iters) the primal state as DIR/<name>.npy (float64; long arrays as a fixed seeded sample)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of --impl ours")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -459,6 +497,9 @@ def main():
         sol.calcdRdWTPsiAD(psi, y)
     barrier()
     e2e_s = (time.perf_counter() - t0) / args.steps
+    outputs = {"dRdWTPsi": y.copy()}  # what the caller of the timed path received in the last step
+    if primal is not None:
+        outputs["primal_states"] = W.copy()
     clocks = sampler.stop() if rank == 0 else None
 
     # max over ranks
@@ -504,7 +545,7 @@ def main():
 
             psi_i, adjoint["idrs"] = leg("IDR(%d)" % args.idr_s, dict(kspType="idrs", idrS=args.idr_s, gmresMaxIters=3 * args.max_iters))
             best = adjoint["idrs"]
-            if not args.no_gmres and (world == 1 or args.gmres_multi):  # the GMRES leg (25 s and a 110 GB basis at 1M cells) runs on one GPU only by default
+            if not args.no_gmres and (world == 1 or args.gmres_multi):  # the GMRES leg runs on one GPU only by default
                 free_b = torch.cuda.mem_get_info()[0]
                 m_fit = int(0.8 * free_b / (8.0 * n)) - 8
                 restart = max(30, min(args.restart, m_fit))
@@ -520,27 +561,19 @@ def main():
             # headline fields = the faster converged leg
             for k in ("method", "wall_s", "solve_s", "fail", "iterations", "rel_residual", "n_matvec"):
                 adjoint[k] = best[k]
+            outputs["adjoint_psi"] = psi_g if best is adjoint.get("gmres") else psi_i
         except Exception as e:  # reported, never hidden
             adjoint = {"error": str(e)}
 
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs, rank, world)
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
         return
 
-    peaks = {}
-    pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(pk):
-        peaks = json.load(open(pk))
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"
-    traffic, traffic_src = None, None
-    tf = os.path.join(ROOT, "profiles", "r02_ncu_kernels_dram.json")
-    if os.path.exists(tf) and world == 1 and not comp:
-        tj = json.load(open(tf))
-        if tj.get("cells") == n_cells_g:
-            traffic = sum(tj[k]["dram__bytes_read.sum"] + tj[k]["dram__bytes_write.sum"] for k in ("RevA", "RevB", "RevC"))
-            traffic_src = "profiles/r02_ncu_kernels_dram.json (ncu dram__bytes_read+write of RevA+RevB+RevC, same workload, commit %s)" % tj.get("commit")
+    peak = 3350.0
+    peak_src = "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
     alg = sol.algorithmicBytes(0)
     achieved = alg / (ms_max * 1e-3) / 1e9
     nC_global = sol.getNGlobalCells()
@@ -550,7 +583,7 @@ def main():
         "warmup": args.warmup, "ms_per_step": ms_max, "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None,
         "dtype": "f64", "data": "synthetic",
         "config": {"workload": "%s %s SA %s %dx%dx%d (%s tiles), %d cells global, %d cells / %d DOF "
-                               "on this GPU; adjoint matvec dRdW^T*psi; working set per product ~%.0f MB >> 126 MB L2 (no explicit flush)"
+                               "on this GPU; adjoint matvec dRdW^T*psi; working set per product ~%.0f MB >> 50 MB L2 (no explicit flush)"
                                % (args.solver, "annular rotor passage (36 per row), cyclic sides + MRF zone," if passage else
                                   ("NACA0012 (linearUpwindV + Spalding wall function)" if args.reference_schemes else "NACA0012"),
                                   "radial x pitchwise x axial" if passage else ("swept tapered wing, 3-D O-grid" if wing else "O-grid, tile-major cell numbering"),
@@ -563,12 +596,13 @@ def main():
                 "h2d_bytes_per_step": 8 * n, "d2h_bytes_per_step": 8 * n,
                 "call": "pyDASolvers.calcdRdWTPsiAD(psi_host, y_host) -> dab_drdwt_mat_vec (pinned host buffers)"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "algorithmic_bytes_per_product": alg,
+                     "peak_source": peak_src, "algorithmic_bytes_per_product": alg,
                      "kernels_ms": per_kernel, "forward_R_ms": ms_fwd,
                      "note": "one product = RevA+RevB+RevC; achieved = algorithmic bytes of the product / its device time"},
         "adjoint_solve": adjoint,
         "primal_solve": primal,
         "clocks": clocks,
+        "device": device_info(local_rank),
     }
     if not args.no_cpu_baseline and world == 1 and not comp and not wing and not passage:
         try:

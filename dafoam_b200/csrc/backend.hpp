@@ -1,4 +1,4 @@
-// Execution backend.  The product build (nvcc, sm_100a) launches every functor as a CUDA kernel on the
+// Execution backend.  The product build (nvcc, sm_90a) launches every functor as a CUDA kernel on the
 // solver's stream.  Defining DAB_HOSTSIM compiles the very same functors into plain host loops: that
 // build exists ONLY so that the non-GPU test suite can check the hand-derived kernels against the
 // oracle on a machine without a GPU (tests/hostsim); it is never loaded by the product package.
@@ -127,7 +127,7 @@ struct Backend
         int n = 0;
         cudaError_t e = cudaGetDeviceCount(&n);
         if (e != cudaSuccess || n == 0)
-            throw Error("dab200 requires a CUDA device (sm_100a); none is visible and there is no CPU fallback");
+            throw Error("dab200 requires a CUDA device (sm_90a); none is visible and there is no CPU fallback");
         DAB_CUDA_CHECK(cudaSetDevice(device));
         DAB_CUDA_CHECK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
         DAB_CUDA_CHECK(cudaStreamCreateWithFlags(&stream2, cudaStreamNonBlocking));

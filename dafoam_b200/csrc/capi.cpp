@@ -1,4 +1,4 @@
-// C ABI of libdab200.so (include/dab200.h).  Compiled by nvcc as CUDA (`-x cu`, sm_100a).
+// C ABI of libdab200.so (include/dab200.h).  Compiled by nvcc as CUDA (`-x cu`, sm_90a).
 #include "../../include/dab200.h"
 #include "solver.hpp"
 #include <cstring>
@@ -54,7 +54,7 @@ const char* dab_version(void)
 #ifdef DAB_HOSTSIM
     return "dab200 0.1 (HOSTSIM test build -- not the product)";
 #else
-    return "dab200 0.1 (sm_100a)";
+    return "dab200 0.1 (sm_90a)";
 #endif
 }
 

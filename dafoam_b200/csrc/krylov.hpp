@@ -184,10 +184,9 @@ struct IluFactorColour
 
 // Triangular solves, one launch per colour.  LANES threads share a cell: the cell's rows (slots) are walked in order -- later rows
 // of the cell read what its earlier rows produced -- and the entries of a row are dealt round-robin to the lanes, the partial sums
-// combined with a shuffle butterfly.  Measured at 1M cells (profiles/r02_adjoint_solve_profile.md): with the multicolour ordering
-// (74k cells per launch) LANES = 1 is FASTER (99 / 76 us per launch against 106 / 105 with 4 lanes): the kernels are bound by the
-// x[col] gathers, which coalesce across the consecutive cells of a warp, and splitting a row over lanes divides that coalescing by
-// LANES.  With the block-natural ordering (40 levels of ~5k cells) 4 lanes win (14.9 -> 11.0 s per solve): there the launches are
+// combined with a shuffle butterfly.  With the multicolour ordering (~74k cells per launch at 1M cells) LANES = 1 is faster: the
+// kernels are bound by the x[col] gathers, which coalesce across the consecutive cells of a warp, and splitting a row over lanes
+// divides that coalescing by LANES.  With the block-natural ordering (levels of ~5k cells) 4 lanes win: there the launches are
 // too small to fill the device.  The ordering picks the variant.
 
 template <int TRI_LANES>
@@ -289,8 +288,8 @@ struct TriUpperColour // x = U^{-1} x, in place; launched over nCells * TRI_LANE
 };
 
 // (Measured and removed: solving a colour in two steps -- one thread per ROW for the other colours' contributions, then one thread per
-// cell for the in-cell substitution -- is slower, 163 + 44 us per colour against 101: the ~10 rows of a cell gather the same x entries,
-// which the per-cell thread re-reads from L1; spread over ten warps they come from L2 ten times.  profiles/r02_adjoint_solve_profile.md)
+// cell for the in-cell substitution -- is slower: the ~10 rows of a cell gather the same x entries, which the per-cell thread
+// re-reads from L1; spread over ten warps they come from L2 ten times.)
 DAB_HD double ellVal(const EllView& A, int64_t o) { return A.valF ? (double)A.valF[o] : A.val[o]; }
 
 // (Also measured and removed: accumulating the other-colour sums of ALL rows of a cell in lock step before the in-cell substitution --
@@ -363,7 +362,7 @@ struct SubVec // r = b - r
 
 #ifndef DAB_HOSTSIM
 constexpr int DOT_TILE = 8;
-constexpr int DOT_BLOCKS = 148 * 4;
+constexpr int DOT_BLOCKS = 132 * 4; // four CTAs on each of an H100's 132 SMs: one even wave
 constexpr int DOT_THREADS = 256;
 // partial[b*k + j] = sum over block b's strided share of V_j . w   (deterministic two-pass reduction)
 __global__ void __launch_bounds__(DOT_THREADS) multiDotPartial(const double* __restrict__ V, int64_t ld, int k, const double* __restrict__ w,

@@ -126,7 +126,7 @@ DAB_HD void boundaryGradAdj(const double* nh, const double* Gbb, double* gUb, do
 }
 
 // ---- face iteration through an accessor: hexahedral meshes (NF = 6) load the cell's whole row of the two tables before the face loop
-// (all index loads in flight together; measured on B200: product 0.855 -> 0.763 ms), other meshes walk the ELL row
+// (all index loads in flight together), other meshes walk the ELL row
 DAB_HD FaceRef faceOfE2(int nIF, int e, int n)
 {
     FaceRef r;

@@ -41,7 +41,7 @@ namespace dab
 #define DAB_FWDB_MINBLOCKS 3
 #endif
 template <int NF, int FEAT> struct LaunchTraits<RevB<NF, FEAT>> { static constexpr int minBlocks = DAB_REVB_MINBLOCKS; };
-// measured with the hoisted load blocks (profiles/r02_kernel_experiments.md): RevA 96 registers / 5 CTAs per SM, RevC 128 / 4
+// with the hoisted load blocks: RevA 96 registers / 5 CTAs per SM, RevC 128 / 4
 template <int NF> struct LaunchTraits<RevA<NF>> { static constexpr int minBlocks = 5; };
 template <int NF> struct LaunchTraits<RevC<NF>> { static constexpr int minBlocks = 4; };
 template <int NF, int FEAT> struct LaunchTraits<FwdB<NF, FEAT>> { static constexpr int minBlocks = DAB_FWDB_MINBLOCKS; };
@@ -53,9 +53,8 @@ template <int NF> struct LaunchTraits<cEEqnAssemble<NF>> { static constexpr int 
 template <int NF> struct LaunchTraits<cNutEqnAssemble<NF>> { static constexpr int minBlocks = 3; };
 template <int NF> struct LaunchTraits<cPEqnAssemble<NF>> { static constexpr int minBlocks = 4; };
 template <int NF> struct LaunchTraits<cPhiUpdate<NF>> { static constexpr int minBlocks = 4; };
-// resident CTAs per SM of the compressible reverse kernels, measured on the 1M-cell DATurboFoam passage (profiles/r02_kernel_experiments.md):
-// cRevA 2 / 3 / 4 CTAs: 0.233 / 0.233 / 0.192 ms; cRevB 2 / 3: 0.581 / 0.551 (168 registers, 1.3 KB of spills, still faster);
-// cRevE (+cRevC) 2 / 3 / 4: 0.823 / 0.639 / 0.592 -- these kernels wait on gathers: more warps beat fewer spills
+// resident CTAs per SM of the compressible reverse kernels: cRevA 4, cRevB 3 (168 registers, with spills), cRevE (+cRevC) 4 --
+// these kernels wait on gathers: more warps beat fewer spills
 #ifndef DAB_CREVA_MINBLOCKS
 #define DAB_CREVA_MINBLOCKS 4
 #endif
@@ -1107,8 +1106,8 @@ struct Solver
     void setupTiles()
     {
         tilesOn = false;
-        // measured on B200 (profiles/r02_tile_kernels.md): the tile kernels are slower than the cell-per-thread kernels (face data
-        // still comes from global memory, one or two CTAs per SM) -- they stay a tested option (DAB_TILE=1), not the default
+        // the tile kernels are slower than the cell-per-thread kernels (face data still comes from global memory, one or two CTAs
+        // per SM) -- they stay a tested option (DAB_TILE=1), not the default
         const char* env = getenv("DAB_TILE");
         if (!env || atoi(env) == 0) return;
         if (partitioned || par.comp || mrf.on || hm.nC < 64) return;
@@ -1152,8 +1151,7 @@ struct Solver
     {
         pfOn = false;
 #ifndef DAB_HOSTSIM
-        // measured on B200 (profiles/r02_kernel_experiments.md, #5): 2-17 % SLOWER at every prefetch distance -- the plans stay an
-        // opt-in measurement hook (DAB_PREFETCH_L2=1), not the default
+        // the plans do not make the product faster -- they stay an opt-in measurement hook (DAB_PREFETCH_L2=1), not the default
         const char* env = getenv("DAB_PREFETCH_L2");
         if (!env || atoi(env) == 0) return;
         const int nC = hm.nC, nIF = hm.nIF;

@@ -15,7 +15,7 @@ namespace dab
 
 // Reciprocal without the slow-path branch of an IEEE fp64 division.  `a / b` compiles to MUFU.RCP64H + Newton steps + a
 // conditional CALL for denormal / huge operands; that branch ends the scheduling region, so the loads of a face stay serialised
-// behind it (the kernels are latency-bound: profiles/r02_latency_analysis.md).  For the operands it is used on (cell volumes,
+// behind it (the kernels are latency-bound).  For the operands it is used on (cell volumes,
 // face areas: normal, positive) two Newton steps on rcp.approx give the correctly rounded result to within 1 ulp.
 DAB_HD double frcp(double x)
 {
@@ -286,9 +286,8 @@ DAB_HD FaceRef faceOfE(const MeshView& m, int e, int n)
 }
 
 // DAB_PREFETCH_IDX (default build): load the cell's whole row of the two ELL tables before the face loop (fixed-size
-// meshes), so that the index loads of all faces are in flight together instead of one dependent round trip per face
-// (measured on B200: product 0.855 -> 0.763 ms).  Requesting the NEXT face's cache lines with prefetch.global.L1 on top of
-// this was measured too and is slower (1.005 ms: the prefetches double the LSU transactions) -- not kept.
+// meshes), so that the index loads of all faces are in flight together instead of one dependent round trip per face.
+// Requesting the NEXT face's cache lines with prefetch.global.L1 on top of this doubles the LSU transactions -- not kept.
 #if defined(DAB_PREFETCH_IDX)
 #define DAB_FACE_PREFETCH(NF)                                                                    \
     int e_[(NF) > 0 ? (NF) : 1], n_[(NF) > 0 ? (NF) : 1];                                        \

@@ -1,12 +1,12 @@
 """PYDAFOAM -- the user-facing class of the reference (dafoam/pyDAFoam.py:673-2200) for the path this package covers,
-on top of the B200 engine: primal (`__call__`), functions, states / volume coordinates, residuals, and the discrete
+on top of the GPU engine: primal (`__call__`), functions, states / volume coordinates, residuals, and the discrete
 adjoint with its total derivatives (what `DAFoamSolver.solve_linear` / `apply_linear` and `DAFoamFunctions.
 compute_jacvec_product` do in dafoam/mphys/mphys_dafoam.py:405-574, 778-792 -- and what the v2/v3 API exposed as
 `solveAdjoint` / `calcTotalDeriv`).
 
 Not reproduced (out of scope, SURVEY.md section 8): OpenMDAO/MPhys components, pyGeo/IDWarp hooks, family groups and
 surface maps, decomposePar, option type checking.  There is no CPU fallback: constructing the object needs
-libdab200.so and a B200."""
+libdab200.so and a CUDA GPU (sm_90a)."""
 from __future__ import annotations
 
 import copy

@@ -4,7 +4,7 @@ Mirrors the reference's Cython class `pyDASolvers` (reference src/pyDASolvers/py
 same method names, same argument meaning (caller-allocated C-contiguous float64 numpy arrays,
 size-asserted), same soft-failure convention (integer returns for solvePrimal/solveLinearEqn, hard
 errors raise).  Implemented as a thin ctypes binding of the C ABI in include/dab200.h; there is no CPU
-fallback: if libdab200.so (CUDA, sm_100a) is missing or no GPU is visible, construction raises.
+fallback: if libdab200.so (CUDA, sm_90a) is missing or no GPU is visible, construction raises.
 
 petsc4py is not available in this environment, so the PETSc handle arguments of the reference
 (`Mat`, `KSP`, `Vec`) are replaced by tiny handle classes defined here (`Mat`, `KSP`) and by plain

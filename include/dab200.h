@@ -1,5 +1,5 @@
 /*
- * dab200.h -- C ABI of the B200-native discrete-adjoint engine (libdab200.so).
+ * dab200.h -- C ABI of the GPU-native discrete-adjoint engine (libdab200.so).
  *
  * This is the drop-in boundary for the adjoint hot path of mdolab/dafoam: each entry point replaces
  * one method of the reference's Cython class `pyDASolvers` (reference src/pyDASolvers/pyDASolvers.pyx:

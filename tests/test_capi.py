@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(L, s), "missing symbol " + s
     L.dab_version.restype = ctypes.c_char_p
-    assert b"sm_100a" in L.dab_version()
+    assert b"sm_90a" in L.dab_version()
 
 
 @pytest.mark.skipif(not os.path.exists(LIB), reason="libdab200.so not built")

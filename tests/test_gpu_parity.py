@@ -1,4 +1,4 @@
-"""-m gpu: the parity tests proper, through the C ABI of the CUDA library (libdab200.so) on a B200."""
+"""-m gpu: the parity tests proper, through the C ABI of the CUDA library (libdab200.so) on an H100."""
 import numpy as np
 import pytest
 
