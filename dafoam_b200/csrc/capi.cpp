@@ -115,6 +115,7 @@ int dab_n_local_adjoint_states(dab_solver* s, int64_t* out) { DAB_TRY need(s, "s
 int dab_n_local_cells(dab_solver* s, int64_t* out) { DAB_TRY need(s, "solver"); *out = s->s.hm.nC; DAB_CATCH }
 int dab_n_global_cells(dab_solver* s, int64_t* out) { DAB_TRY need(s, "solver"); *out = s->s.part.nGlobalCells; DAB_CATCH }
 int dab_n_local_points(dab_solver* s, int64_t* out) { DAB_TRY need(s, "solver"); *out = s->s.hm.nP; DAB_CATCH }
+int dab_volcoord_evaluations(dab_solver* s, int64_t* out) { DAB_TRY need(s, "solver"); *out = s->s.volc.nEval; DAB_CATCH }
 int dab_n_local_faces(dab_solver* s, int64_t* out) { DAB_TRY need(s, "solver"); *out = s->s.hm.nF; DAB_CATCH }
 int dab_n_local_internal_faces(dab_solver* s, int64_t* out) { DAB_TRY need(s, "solver"); *out = s->s.hm.nIF; DAB_CATCH }
 

@@ -151,14 +151,22 @@ struct Comm
 // ---- pack / unpack kernels ---------------------------------------------------------------------------------
 // component k of an exchanged item at `cell`, as the receiver must see it.  xs != 0: the value crosses a cyclic patch pair whose
 // transform is R = Rtab[|xs| - 1] (xs < 0: the inverse, R^T): 3-component items are vectors (v' = R v), 9-component items rank-2
-// tensors (T' = R T R^T; gradients and their adjoints), everything else is a scalar.  Role of OpenFOAM's
-// cyclicFvPatchField::patchNeighbourField -> transform(forwardT(), pnf).
-DAB_HD double haloValue(const double* arr, int64_t cell, int cellStride, int compStride, int ncomp, int k, int xs, const double* Rtab)
+// tensors (T' = R T R^T; gradients and their adjoints), everything else is a scalar.  Ttab != nullptr marks a 3-component item as a
+// position (cell centres): x' = R x + t with t = Ttab[3 (|xs| - 1)], inverse x' = R^T (x - t) (HostMesh::xfPoint, the same operation
+// order).  Role of OpenFOAM's cyclicFvPatchField::patchNeighbourField -> transform(forwardT(), pnf).
+DAB_HD double haloValue(const double* arr, int64_t cell, int cellStride, int compStride, int ncomp, int k, int xs, const double* Rtab,
+                        const double* Ttab = nullptr)
 {
     const double* a = arr + cell * cellStride;
     if (xs == 0 || (ncomp != 3 && ncomp != 9)) return a[(int64_t)k * compStride];
     const double* M = Rtab + 9 * ((xs < 0 ? -xs : xs) - 1);
     const bool inv = xs < 0;
+    if (ncomp == 3 && Ttab)
+    {
+        const double* t = Ttab + 3 * ((xs < 0 ? -xs : xs) - 1);
+        if (!inv) return M[3 * k] * a[0] + M[3 * k + 1] * a[compStride] + M[3 * k + 2] * a[2 * (int64_t)compStride] + t[k];
+        return M[k] * (a[0] - t[0]) + M[3 + k] * (a[compStride] - t[1]) + M[6 + k] * (a[2 * (int64_t)compStride] - t[2]);
+    }
     if (ncomp == 3)
     {
         double v = 0.0;
@@ -185,11 +193,12 @@ struct HaloPack
     double* buf;
     const int32_t* xf = nullptr; // [nSend] signed cyclic transform of the element (nullptr: none anywhere)
     const double* Rtab = nullptr;
+    const double* Ttab = nullptr; // translations: the item is a position (see haloValue)
     DAB_HD void operator()(int i) const
     {
         const int k = i / nSend, j = i - k * nSend;
         const int64_t o = (int64_t)segOff[j] * sumComp + (int64_t)(compBase + k) * segCnt[j] + (j - segOff[j]);
-        buf[o] = haloValue(arr, idx[j], cellStride, compStride, ncomp, k, xf ? xf[j] : 0, Rtab);
+        buf[o] = haloValue(arr, idx[j], cellStride, compStride, ncomp, k, xf ? xf[j] : 0, Rtab, Ttab);
     }
 };
 // couplings of a rank with itself (cyclic patch pair inside one sub-mesh): ghost slot <- transformed value of the local cell
@@ -200,10 +209,11 @@ struct SelfCopy
     const int32_t *src, *dst, *xf; // [n]; xf may be nullptr (faces)
     int n;
     const double* Rtab;
+    const double* Ttab; // translations: the item is a position (see haloValue)
     DAB_HD void operator()(int i) const
     {
         const int k = i / n, j = i - k * n;
-        arr[(int64_t)dst[j] * cellStride + (int64_t)k * compStride] = haloValue(arr, src[j], cellStride, compStride, ncomp, k, xf ? xf[j] : 0, Rtab);
+        arr[(int64_t)dst[j] * cellStride + (int64_t)k * compStride] = haloValue(arr, src[j], cellStride, compStride, ncomp, k, xf ? xf[j] : 0, Rtab, Ttab);
     }
 };
 struct HaloUnpack
@@ -238,6 +248,7 @@ struct P2pItems
     int n, sumComp;
     double* arr[P2P_MAXITEMS];
     int cellStride[P2P_MAXITEMS], compStride[P2P_MAXITEMS], ncomp[P2P_MAXITEMS], compBase[P2P_MAXITEMS];
+    bool position[P2P_MAXITEMS];
 };
 struct P2pDst
 {
@@ -252,14 +263,15 @@ struct P2pPack
     const int32_t *idx, *segOff, *segCnt, *peerOf; // [nSend]
     int nSend;
     const int32_t* xf;  // [nSend] signed cyclic transform (nullptr: none anywhere)
-    const double* Rtab;
+    const double *Rtab, *Ttab;
     __device__ void operator()(int t) const
     {
         const int kk = t / nSend, j = t - kk * nSend;
         int a = 0;
         while (a + 1 < it.n && kk >= it.compBase[a + 1]) a++;
         const int k = kk - it.compBase[a];
-        const double v = haloValue(it.arr[a], idx[j], it.cellStride[a], it.compStride[a], it.ncomp[a], k, xf ? xf[j] : 0, Rtab);
+        const double v = haloValue(it.arr[a], idx[j], it.cellStride[a], it.compStride[a], it.ncomp[a], k, xf ? xf[j] : 0, Rtab,
+                                   it.position[a] ? Ttab : nullptr);
         dst.base[peerOf[j]][(int64_t)kk * segCnt[j] + (j - segOff[j])] = v;
     }
 };
@@ -382,6 +394,7 @@ struct HaloItem
 {
     double* arr;
     int ncomp, cellStride, compStride;
+    bool position = false; // a 3-component position: crosses a cyclic pair with the translation as well (haloValue)
 };
 
 struct Halo
@@ -525,7 +538,7 @@ struct Halo
         for (int i = 0; i < it.n; i++)
         {
             it.arr[i] = items[i].arr; it.cellStride[i] = items[i].cellStride; it.compStride[i] = items[i].compStride;
-            it.ncomp[i] = items[i].ncomp; it.compBase[i] = base;
+            it.ncomp[i] = items[i].ncomp; it.compBase[i] = base; it.position[i] = items[i].position;
             base += items[i].ncomp;
         }
         P2pDst dst;
@@ -534,7 +547,7 @@ struct Halo
             dst.base[p] = peerWin[p] + peerData[st][q][p] + (size_t)peerRecvOff[st][p] * sumComp;
             dst.flag[p] = (long long*)(peerWin[p] + peerFlag[st][q][p]) + myIdxInPeer[p];
         }
-        if (hs.nSend > 0) be->launch(hs.nSend * sumComp, P2pPack{it, dst, hs.dSendIdx.p, hs.dSendSegOff.p, hs.dSendSegCnt.p, hs.dSendPeer.p, hs.nSend, hs.xfPtr(), dRtab.p});
+        if (hs.nSend > 0) be->launch(hs.nSend * sumComp, P2pPack{it, dst, hs.dSendIdx.p, hs.dSendSegOff.p, hs.dSendSegCnt.p, hs.dSendPeer.p, hs.nSend, hs.xfPtr(), dRtab.p, dTtab.p});
         p2pSignal<<<1, 32, 0, be->stream>>>(dst, nP, hs.epoch);
         const int n = hs.nRecv * sumComp;
         if (n > 0)
@@ -550,6 +563,7 @@ struct Halo
 #endif
 
     DevBuf<double> dRtab; // rotation matrices of the cyclic transforms, 9 doubles each
+    DevBuf<double> dTtab; // their translations, 3 doubles each
     bool remote() const { return comm && comm->active(); }
     bool any() const { return remote() || cells.nSelf > 0 || faces.nSelf > 0; }
 
@@ -558,10 +572,14 @@ struct Halo
         be = &b;
         comm = &c;
         peers = plan.peers;
-        std::vector<double> R(9 * xforms.size() + 1, 0.0);
+        std::vector<double> R(9 * xforms.size() + 1, 0.0), T(3 * xforms.size() + 1, 0.0);
         for (size_t k = 0; k < xforms.size(); k++)
+        {
             for (int a = 0; a < 9; a++) R[9 * k + a] = xforms[k].R[a];
+            for (int a = 0; a < 3; a++) T[3 * k + a] = xforms[k].t[a];
+        }
         dRtab.upload(b, R);
+        dTtab.upload(b, T);
         std::vector<std::vector<int32_t>> recvCells(plan.peers.size());
         for (size_t p = 0; p < plan.peers.size(); p++)
             for (int i = 0; i < plan.recvCellCount[p]; i++) recvCells[p].push_back(plan.recvCellStart[p] + i);
@@ -580,7 +598,7 @@ struct Halo
         if (hs.nSelf == 0) return;
         for (const auto& it : items)
             be->launch(hs.nSelf * it.ncomp, SelfCopy{it.arr, it.cellStride, it.compStride, it.ncomp, hs.dSelfSrc.p, hs.dSelfDst.p,
-                                                     hs.dSelfXf.n ? hs.dSelfXf.p : nullptr, hs.nSelf, dRtab.p});
+                                                     hs.dSelfXf.n ? hs.dSelfXf.p : nullptr, hs.nSelf, dRtab.p, it.position ? dTtab.p : nullptr});
     }
 
     void run(HaloSet& hs, const std::vector<HaloItem>& items)
@@ -602,7 +620,8 @@ struct Halo
         for (const auto& it : items)
         {
             be->launch(hs.nSend * it.ncomp, HaloPack{it.arr, it.cellStride, it.compStride, it.ncomp, hs.dSendIdx.p, hs.dSendSegOff.p,
-                                                     hs.dSendSegCnt.p, hs.nSend, sumComp, base, hs.sendBuf.p, hs.xfPtr(), dRtab.p});
+                                                     hs.dSendSegCnt.p, hs.nSend, sumComp, base, hs.sendBuf.p, hs.xfPtr(), dRtab.p,
+                                                     it.position ? dTtab.p : nullptr});
             base += it.ncomp;
         }
         std::vector<const double*> sb;
@@ -663,7 +682,8 @@ struct Halo
         for (const auto& it : items)
         {
             be->launch(hs.nSend * it.ncomp, HaloPack{it.arr, it.cellStride, it.compStride, it.ncomp, hs.dSendIdx.p, hs.dSendSegOff.p,
-                                                     hs.dSendSegCnt.p, hs.nSend, sumComp, base, hs.sendBuf.p, hs.xfPtr(), dRtab.p});
+                                                     hs.dSendSegCnt.p, hs.nSend, sumComp, base, hs.sendBuf.p, hs.xfPtr(), dRtab.p,
+                                                     it.position ? dTtab.p : nullptr});
             base += it.ncomp;
         }
         cudaEventRecord(hs.evPack, be->stream);

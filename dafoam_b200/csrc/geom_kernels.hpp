@@ -22,6 +22,10 @@ struct GeomView
     const int32_t *fOff, *fLab, *own, *nei, *cellFaces;
     const double* pts; // [3*nP]
     double *Sx, *Sy, *Sz, *magSf, *w, *delta, *kx, *ky, *kz, *Cfx, *Cfy, *Cfz, *Cx, *Cy, *Cz, *V;
+    // partitioned local mesh with cyclic pairs: faceXf[f] = k > 0 puts face f into the neighbour's frame (inverse of transform k,
+    // rotations Rtab / translations Ttab as in comm.hpp); nullptr: no such face
+    const int32_t* faceXf;
+    const double *Rtab, *Ttab;
 };
 
 // face area vector and centroid (primitiveMesh::makeFaceCentresAndAreas)
@@ -82,13 +86,27 @@ struct GeomFaceK
                 sf[k] = 0.5 * sumN[k];
             }
         }
+        g.magSf[f] = sqrt(sf[0] * sf[0] + sf[1] * sf[1] + sf[2] * sf[2]);
+        const int x = g.faceXf ? g.faceXf[f] : 0;
+        if (x > 0)
+        {
+            // the neighbour-side copy of a coupled face (HostMesh::xfPoint / xfVector, inverse, the same operation order)
+            const double* M = g.Rtab + 9 * (x - 1);
+            const double* t = g.Ttab + 3 * (x - 1);
+            const double d[3] = {cf[0] - t[0], cf[1] - t[1], cf[2] - t[2]}, s0[3] = {sf[0], sf[1], sf[2]};
+            for (int a = 0; a < 3; a++)
+            {
+                cf[a] = M[a] * d[0] + M[3 + a] * d[1] + M[6 + a] * d[2];
+                sf[a] = M[a] * s0[0] + M[3 + a] * s0[1] + M[6 + a] * s0[2];
+            }
+        }
         g.Cfx[f] = cf[0]; g.Cfy[f] = cf[1]; g.Cfz[f] = cf[2];
         g.Sx[f] = sf[0]; g.Sy[f] = sf[1]; g.Sz[f] = sf[2];
-        g.magSf[f] = sqrt(sf[0] * sf[0] + sf[1] * sf[1] + sf[2] * sf[2]);
     }
 };
 
-// cell centroid and volume from the face pyramids (primitiveMesh::makeCellCentresAndVols)
+// cell centroid and volume from the face pyramids (primitiveMesh::makeCellCentresAndVols); owned cells only -- on a partitioned
+// mesh the ghost cells' centres and volumes come from their owners through the halo (centres as positions)
 struct GeomCellK
 {
     GeomView g;
@@ -192,32 +210,35 @@ struct PointMove
     }
 };
 
-// footprint labels: label[c] = home cell whose ball c lies in (-1: none); one propagation sweep
+// footprint labels: label[c] = global id of the home cell whose ball c lies in (-1: none), over owned and ghost cells; doubles,
+// so that a partitioned mesh refreshes the ghost labels through the halo after every sweep (the ids are exact integers)
 struct LabelInit
 {
-    int32_t* label;
-    DAB_HD void operator()(int c) const { label[c] = -1; }
+    double* label;
+    DAB_HD void operator()(int c) const { label[c] = -1.0; }
 };
 struct LabelSeed
 {
-    int32_t* label;
-    const int32_t* homes;
-    DAB_HD void operator()(int t) const { label[homes[t]] = homes[t]; }
+    double* label;
+    const int32_t* cells; // local cells (owned or ghost) that are homes of the colour
+    const int32_t* ids;   // their global ids
+    DAB_HD void operator()(int t) const { label[cells[t]] = (double)ids[t]; }
 };
+// one propagation sweep over the owned cells
 struct LabelSweep
 {
-    const int32_t* in;
-    int32_t* out;
+    const double* in;
+    double* out;
     const int32_t* cellNbr;
     int nC, maxCF;
     DAB_HD void operator()(int c) const
     {
-        int l = in[c];
-        if (l < 0)
+        double l = in[c];
+        if (l < 0.0)
             for (int k = 0; k < maxCF; k++)
             {
                 const int n = cellNbr[(size_t)k * nC + c];
-                if (n >= 0 && n < nC && in[n] > l) l = in[n];
+                if (n >= 0 && in[n] > l) l = in[n];
             }
         out[c] = l;
     }
@@ -238,14 +259,14 @@ struct VolCoordAccumR
     MeshView m;
     int ns, offPhi; // cell-state rows: U (3 per cell, AoS) then ns-3 scalar blocks; face rows from offPhi
     const double *Rp, *Rm, *psi;
-    const int32_t* label;
-    const int32_t* slotPoint; // [nC*maxSlots]
+    const double* label;
+    const int32_t* slotPoint; // [global cells * maxSlots]
     int maxSlots, slot, k;
     const double* eps;
     double* out;
     DAB_HD void operator()(int c) const
     {
-        const int h = label[c];
+        const int h = (int)label[c];
         if (h < 0) return;
         const int p = slotPoint[(size_t)h * maxSlots + slot];
         if (p < 0) return;
@@ -270,7 +291,7 @@ struct VolCoordAccumF
 {
     MeshView m;
     const double *Fp, *Fm; // [nBF]
-    const int32_t* label;
+    const double* label;
     const int32_t* slotPoint;
     int maxSlots, slot, k;
     const double* eps;
@@ -279,7 +300,7 @@ struct VolCoordAccumF
     DAB_HD void operator()(int b) const
     {
         const int c = m.own[m.nIF + b];
-        const int h = label[c];
+        const int h = (int)label[c];
         if (h < 0) return;
         const int p = slotPoint[(size_t)h * maxSlots + slot];
         if (p < 0) return;

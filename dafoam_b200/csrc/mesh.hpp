@@ -36,6 +36,9 @@ struct HostMesh
     struct CycXf { double R[9]; double t[3]; };
     std::vector<int32_t> cyc;            // per internal face (global mesh only); empty = no cyclic faces
     std::vector<CycXf> xforms;           // transform k is xforms[k - 1]
+    // the coupled face pairs as read, for the check of moved points (checkCyclicPairs): pair i has the points of the first-patch face
+    // cycA[cycAOff[i]..] and of the second-patch face cycB[cycBOff[i]..] and the transform cycXf[i]; kept by every local mesh
+    std::vector<int32_t> cycAOff, cycA, cycBOff, cycB, cycXf;
     bool hasCyclic() const { return !xforms.empty(); }
     static void xfPoint(const CycXf& X, bool inverse, const double* x, double* y)
     {
@@ -70,11 +73,10 @@ struct HostMesh
     }
 
     // centre and area vector of face f from its points (OpenFOAM primitiveMeshFaceCentresAndAreas)
-    void faceGeom(int f, double* cf, double* sf) const
+    void faceGeom(int f, double* cf, double* sf) const { polyGeom(&fLab[fOff[f]], fOff[f + 1] - fOff[f], cf, sf); }
+    void polyGeom(const int32_t* l, int n, double* cf, double* sf) const
     {
         const double* P = points.data();
-        const int n = fOff[f + 1] - fOff[f];
-        const int32_t* l = &fLab[fOff[f]];
         if (n == 3)
         {
             for (int k = 0; k < 3; k++) cf[k] = (P[3 * l[0] + k] + P[3 * l[1] + k] + P[3 * l[2] + k]) / 3.0;
@@ -102,6 +104,38 @@ struct HostMesh
         for (int k = 0; k < 3; k++) { cf[k] = (1.0 / 3.0) / sumA * sumAc[k]; sf[k] = 0.5 * sumN[k]; }
     }
 
+    // the read-time rule of a coupled pair: the transform maps the second face onto the first (centres coincide, area vectors opposite)
+    static bool pairMatches(const CycXf& X, const double* cA, const double* sA, const double* cB, const double* sB, double scale)
+    {
+        double y[3], v[3], mA = 0.0;
+        xfPoint(X, false, cB, y);
+        xfVector(X, false, sB, v);
+        for (int a = 0; a < 3; a++) mA = std::max(mA, std::fabs(sA[a]));
+        for (int a = 0; a < 3; a++)
+            if (std::fabs(y[a] - cA[a]) > 1e-6 * scale || std::fabs(v[a] + sA[a]) > 1e-6 * mA) return false;
+        return true;
+    }
+    double pointScale() const
+    {
+        double scale = 0.0;
+        for (size_t i = 0; i < points.size(); i++) scale = std::max(scale, std::fabs(points[i]));
+        return scale;
+    }
+    // moved points (updateOFMesh): every coupled pair must still match under its (fixed) transform, i.e. the displacement is periodic
+    void checkCyclicPairs() const
+    {
+        const double scale = pointScale();
+        for (size_t i = 0; i + 1 < cycAOff.size(); i++)
+        {
+            double cA[3], sA[3], cB[3], sB[3];
+            polyGeom(&cycA[cycAOff[i]], cycAOff[i + 1] - cycAOff[i], cA, sA);
+            polyGeom(&cycB[cycBOff[i]], cycBOff[i + 1] - cycBOff[i], cB, sB);
+            if (!pairMatches(xforms[cycXf[i] - 1], cA, sA, cB, sB, scale))
+                throw Error("updateOFMesh: coupled face pair " + std::to_string(i) + " of cyclic transform " + std::to_string(cycXf[i])
+                            + " no longer matches under the patch transform (the displacement must be periodic)");
+        }
+    }
+
     // Cyclic patch pairs -> internal faces (OpenFOAM cyclicPolyPatch: face i of a patch is coupled to face i of its neighbourPatch;
     // DAFoam counts both sides as coupled boundary faces with a phi state each, reference src/adjoint/DAIndex/DAIndex.C:151-167 --
     // here a pair shares ONE face and one phi state, like the cut faces between ranks).  The transform is taken from the geometry of
@@ -123,8 +157,7 @@ struct HostMesh
         std::vector<int32_t> newOwn(own.begin(), own.begin() + nIF0), newNei(nei), newCyc(nIF0, 0);
         std::vector<int> faceOrder(nIF0);
         for (int f = 0; f < nIF0; f++) faceOrder[f] = f;
-        double scale = 0.0;
-        for (size_t i = 0; i < points.size(); i++) scale = std::max(scale, std::fabs(points[i]));
+        const double scale = pointScale();
         for (size_t p = 0; p < patches.size(); p++)
         {
             if (!isCyc[p]) continue;
@@ -192,19 +225,20 @@ struct HostMesh
             }
             // every coupled pair must map onto each other: centres coincide, area vectors are opposite
             for (int i = 0; i < n; i++)
-            {
-                double y[3], v[3];
-                xfPoint(X, false, &cB[3 * (size_t)i], y);
-                xfVector(X, false, &sB[3 * (size_t)i], v);
-                double mA = 0.0;
-                for (int a = 0; a < 3; a++) mA = std::max(mA, std::fabs(sA[3 * (size_t)i + a]));
-                for (int a = 0; a < 3; a++)
-                    if (std::fabs(y[a] - cA[3 * (size_t)i + a]) > 1e-6 * scale || std::fabs(v[a] + sA[3 * (size_t)i + a]) > 1e-6 * mA)
-                        throw Error("polyMesh: faces " + std::to_string(i) + " of cyclic patches " + A.name + " / " + B.name
-                                    + " do not match under the patch transform (ordering or transform entry)");
-            }
+                if (!pairMatches(X, &cA[3 * (size_t)i], &sA[3 * (size_t)i], &cB[3 * (size_t)i], &sB[3 * (size_t)i], scale))
+                    throw Error("polyMesh: faces " + std::to_string(i) + " of cyclic patches " + A.name + " / " + B.name
+                                + " do not match under the patch transform (ordering or transform entry)");
             xforms.push_back(X);
             const int k = (int)xforms.size();
+            if (cycAOff.empty()) { cycAOff.push_back(0); cycBOff.push_back(0); }
+            for (int i = 0; i < n; i++)
+            {
+                for (int q = fOff[A.start + i]; q < fOff[A.start + i + 1]; q++) cycA.push_back(fLab[q]);
+                for (int q = fOff[B.start + i]; q < fOff[B.start + i + 1]; q++) cycB.push_back(fLab[q]);
+                cycAOff.push_back((int32_t)cycA.size());
+                cycBOff.push_back((int32_t)cycB.size());
+                cycXf.push_back(k);
+            }
             for (int i = 0; i < n; i++)
             {
                 newOwn.push_back(own[A.start + i]);

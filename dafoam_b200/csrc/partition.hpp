@@ -35,6 +35,7 @@ struct Partition
     std::vector<int32_t> cellGlobal; // local (owned + ghost) -> global cell
     std::vector<int32_t> faceGlobal; // local face -> global face
     std::vector<uint8_t> faceOwned;  // 1 if the phi DOF of the local face belongs to this rank
+    std::vector<int32_t> faceXf;     // k > 0: the local face is the neighbour-side copy of a face of cyclic transform k (geometry in that frame)
     HaloPlan halo;
 };
 
@@ -269,6 +270,9 @@ inline void extractLocalMesh(const HostMesh& g, const std::vector<int>& part, in
         l.fOff.push_back((int32_t)l.fLab.size());
     }
     l.xforms = g.xforms;
+    l.cycAOff = g.cycAOff; l.cycA = g.cycA; l.cycBOff = g.cycBOff; l.cycB = g.cycB; l.cycXf = g.cycXf;
+    P.faceXf.assign(nF, 0);
+    for (int i = nA + nB; i < nIF; i++) P.faceXf[i] = cycOf(lf[i]);
     l.patchGeom = g.patchGeom;
     l.bPatch.assign(l.nBF, -1);
     for (size_t p = 0; p < l.patches.size(); p++)

@@ -183,10 +183,16 @@ struct VolCoord
     bool ready = false;
     int radius = 6;         // residual rows within `radius` cells of a point's home cell may depend on the point
     double relStep = 3e-5;  // finite-difference step relative to the shortest edge at the point
-    int nColours = 0, maxSlots = 1;
+    int nColours = 0, maxSlots = 1, nEval = 0; // nEval: residual evaluations per product
+    // the colouring is computed on the global mesh, so that every rank moves the same points in the same evaluation; homeStart
+    // indexes this rank's seed cells (local owned or ghost cells that are homes) per colour, listStart the global points per (colour, slot)
     std::vector<int> homeStart, listStart;
-    DevBuf<int32_t> dFOff, dFLab, dSlotPoint, dHomes, dLists, dLabelA, dLabelB;
-    DevBuf<double> dEps, dPts, dPts0, dR2, dOut, dF1, dF2;
+    DevBuf<int32_t> dSlotPoint, dHomes, dHomeIds, dLists;
+    DevBuf<double> dEps, dPts0, dR2, dOut, dF1, dF2, dLabelA, dLabelB;
+    // device geometry pipeline (deviceGeometry): face -> point lists of the local mesh and the points it reads
+    bool topoReady = false;
+    DevBuf<int32_t> dFOff, dFLab, dFaceXf;
+    DevBuf<double> dPts;
 };
 
 struct Solver
@@ -247,7 +253,8 @@ struct Solver
 
     // device mesh
     DevBuf<int32_t> dOwn, dNei, dCellFaces, dCellNbr, dBPatch;
-    DevBuf<double> dS[3], dMagSf, dW, dDelta, dK[3], dCf[3], dC[3], dV, dY;
+    DevBuf<double> dS[3], dMagSf, dW, dDelta, dK[3], dCf[3], dV, dY;
+    DevBuf<double> dC; // cell centres, SoA in one buffer (x | y | z, nCtot each): one halo item when the geometry is rebuilt
     MeshView mv;
     // state (internal working copies with ghost slots) and external-layout mirror
     DevBuf<double> dWext, dU, dP, dNt, dPhi, dT;
@@ -1038,8 +1045,9 @@ struct Solver
             dS[k].upload(be, hm.Sf[k]);
             dK[k].upload(be, hm.corr[k]);
             dCf[k].upload(be, hm.Cf[k]);
-            dC[k].upload(be, hm.C[k]);
         }
+        dC.alloc(be, (size_t)3 * hm.nCtot, false);
+        for (int k = 0; k < 3; k++) be.h2d(dC.p + (size_t)k * hm.nCtot, hm.C[k].data(), (size_t)hm.nCtot * sizeof(double));
         dMagSf.upload(be, hm.magSf);
         dW.upload(be, hm.w);
         dDelta.upload(be, hm.delta);
@@ -1049,7 +1057,7 @@ struct Solver
         mv.own = dOwn.p; mv.nei = dNei.p; mv.cellFaces = dCellFaces.p; mv.cellNbr = dCellNbr.p; mv.bPatch = dBPatch.p;
         mv.Sx = dS[0].p; mv.Sy = dS[1].p; mv.Sz = dS[2].p; mv.magSf = dMagSf.p; mv.w = dW.p; mv.delta = dDelta.p;
         mv.kx = dK[0].p; mv.ky = dK[1].p; mv.kz = dK[2].p; mv.Cfx = dCf[0].p; mv.Cfy = dCf[1].p; mv.Cfz = dCf[2].p;
-        mv.Cx = dC[0].p; mv.Cy = dC[1].p; mv.Cz = dC[2].p; mv.V = dV.p; mv.yWall = dY.p;
+        mv.Cx = dC.p; mv.Cy = dC.p + hm.nCtot; mv.Cz = dC.p + 2 * (size_t)hm.nCtot; mv.V = dV.p; mv.yWall = dY.p;
         mv.fvS = nullptr;
         mv.mrfCell = nullptr; mv.mrfType = nullptr; mv.mrfFlux = nullptr;
         if (mrf.on)
@@ -2379,6 +2387,8 @@ struct Solver
     // ---- mesh coordinates as an input (volCoord) ------------------------------------------------------
     VolCoord volc;
     void uploadGeometry();
+    void deviceGeometry();
+    void downloadGeometry();
     void updateMesh(const double* pts);
     void volCoordSetup();
     void volCoordProduct(const double* psi, const FunctionDef* function, double seed, double* out);

@@ -179,6 +179,10 @@ class pyDASolvers:
     def getNLocalPoints(self):
         return self._geti(self._L.dab_n_local_points)
 
+    def getVolCoordEvaluations(self):
+        """residual evaluations of one volCoord product (colouring of the first product; the same on every rank)"""
+        return self._geti(self._L.dab_volcoord_evaluations)
+
     def getNLocalFaces(self):
         return self._geti(self._L.dab_n_local_faces)
 
@@ -400,13 +404,13 @@ class pyDASolvers:
         return nCellStates * (self.getNLocalFaces() - self.getNLocalInternalFaces())
 
     def setGlobalXvOffset(self, offset):
-        """Several ranks: the sum of 3*nLocalPoints over the lower ranks (the caller owns the communicator)."""
+        """Offset added to the volCoord indices (default 0).  Every rank holds the full point list and its volCoord products are
+        summed over the ranks (the distributed-input convention), so the index of a point is the same on every rank; a caller that
+        lays the ranks' point vectors end to end passes the sum of 3*nLocalPoints over the lower ranks instead."""
         self._xvOffset = int(offset)
 
     def getGlobalXvIndex(self, pointI, coordI):
-        """Reference DAIndex.C:704-733: rank offset + pointI*3 + coordI."""
-        if self._nRanks > 1 and not hasattr(self, "_xvOffset"):
-            raise DAB200Error("getGlobalXvIndex on several ranks: call setGlobalXvOffset(sum of 3*nLocalPoints of the lower ranks) first")
+        """Reference DAIndex.C:704-733: offset + pointI*3 + coordI."""
         assert 0 <= pointI < self.getNLocalPoints() and 0 <= coordI < 3
         return getattr(self, "_xvOffset", 0) + 3 * pointI + coordI
 

@@ -101,6 +101,8 @@ int dab_n_local_adjoint_states(dab_solver* s, int64_t* out);
 int dab_n_local_cells(dab_solver* s, int64_t* out);
 int dab_n_global_cells(dab_solver* s, int64_t* out);
 int dab_n_local_points(dab_solver* s, int64_t* out);
+/* residual evaluations of one volCoord product (0 before the first product); the same on every rank */
+int dab_volcoord_evaluations(dab_solver* s, int64_t* out);
 int dab_n_local_faces(dab_solver* s, int64_t* out);
 int dab_n_local_internal_faces(dab_solver* s, int64_t* out);
 
