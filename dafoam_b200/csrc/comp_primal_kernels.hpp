@@ -64,7 +64,8 @@ struct cUEqnAssemble
                 {
                     const bool ownUp = s.phi[f] > 0.0;
                     const bool cUp = fr.s > 0 ? ownUp : !ownUp;
-                    const double* gu = cUp ? gUc : gUn;
+                    double gu[9]; // per-element selects: a pointer into either array would put both in local memory
+                    for (int i = 0; i < 9; i++) gu[i] = cUp ? gUc[i] : gUn[i];
                     const int u = cUp ? c : n;
                     const double d[3] = {m.Cfx[f] - m.Cx[u], m.Cfy[f] - m.Cy[u], m.Cfz[f] - m.Cz[u]};
                     double corr[3];
@@ -81,12 +82,15 @@ struct cUEqnAssemble
                 }
                 const double kv[3] = {m.kx[f], m.ky[f], m.kz[f]};
                 const double wo = m.w[f];
-                const double* gO = fr.s > 0 ? gUc : gUn;
-                const double* gN_ = fr.s > 0 ? gUn : gUc;
+                const bool own = fr.s > 0; // value selects: a pointer into either gradient array would put both in local memory
                 for (int j = 0; j < 3; j++)
                 {
                     double cg = 0.0;
-                    for (int i = 0; i < 3; i++) cg += kv[i] * (wo * gO[j * 3 + i] + (1.0 - wo) * gN_[j * 3 + i]);
+                    for (int i = 0; i < 3; i++)
+                    {
+                        const double gO = own ? gUc[j * 3 + i] : gUn[j * 3 + i], gN_ = own ? gUn[j * 3 + i] : gUc[j * 3 + i];
+                        cg += kv[i] * (wo * gO + (1.0 - wo) * gN_);
+                    }
                     X[j] -= fr.s * gf * cg;
                 }
                 const double trn = gUn[0] + gUn[4] + gUn[8];

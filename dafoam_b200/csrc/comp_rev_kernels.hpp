@@ -356,7 +356,8 @@ struct cRevB
                     }
                     if (schU == DIV_LINEAR_UPWIND || schU == DIV_LINEAR_UPWIND_V)
                     {
-                        const double* gu = cUp ? gUc : gUn;
+                        double gu[9]; // per-element selects: a pointer into either array would put both in local memory
+                        for (int i = 0; i < 9; i++) gu[i] = cUp ? gUc[i] : gUn[i];
                         const int u = cUp ? c : n;
                         const double d[3] = {m.Cfx[f] - m.Cx[u], m.Cfy[f] - m.Cy[u], m.Cfz[f] - m.Cz[u]};
                         double corr[3], corrL[3], outb[3], corrb[3] = {0, 0, 0};

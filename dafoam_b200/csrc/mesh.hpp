@@ -310,6 +310,8 @@ struct HostMesh
         maxCF = *std::max_element(cnt.begin(), cnt.end());
         cellFaces.assign((size_t)maxCF * nC, -1);
         std::fill(cnt.begin(), cnt.end(), 0);
+        // rows filled in ascending face id, and boundary ids are >= nIF: every row is [internal..., boundary..., -1 padding]
+        // (checkEllOrder).  RevB walks a row in two passes on this invariant (rev_kernels.hpp)
         for (int f = 0; f < nF; f++)
         {
             int c = own[f];
@@ -318,6 +320,23 @@ struct HostMesh
             {
                 c = nei[f];
                 cellFaces[(size_t)cnt[c]++ * nC + c] = (f << 1) | 1;
+            }
+        }
+        checkEllOrder();
+    }
+
+    // every ELL row lists its internal faces, then its boundary faces, then padding
+    void checkEllOrder() const
+    {
+        for (int c = 0; c < nC; c++)
+        {
+            int stage = 0; // 0 internal, 1 boundary, 2 padding
+            for (int k = 0; k < maxCF; k++)
+            {
+                const int e = cellFaces[(size_t)k * nC + c];
+                const int s = e < 0 ? 2 : ((e >> 1) >= nIF ? 1 : 0);
+                if (s < stage) throw Error("mesh: ELL row of cell " + std::to_string(c) + " is not ordered internal, boundary, padding");
+                stage = s;
             }
         }
     }

@@ -287,11 +287,14 @@ inline void extractLocalMesh(const HostMesh& g, const std::vector<int>& part, in
     l.maxCF = nC ? *std::max_element(cnt.begin(), cnt.end()) : 0;
     l.cellFaces.assign((size_t)l.maxCF * nC, -1);
     std::fill(cnt.begin(), cnt.end(), 0);
+    // ascending local face id, boundary ids >= nIF (cut faces are internal faces with a ghost neighbour): every row is
+    // [internal..., boundary..., -1 padding], the order RevB's two passes over a row rely on
     for (int i = 0; i < nF; i++)
     {
         if (l.own[i] < nC) l.cellFaces[(size_t)cnt[l.own[i]]++ * nC + l.own[i]] = (i << 1);
         if (i < nIF && l.nei[i] < nC) l.cellFaces[(size_t)cnt[l.nei[i]]++ * nC + l.nei[i]] = (i << 1) | 1;
     }
+    l.checkEllOrder();
     // geometry slices
     for (int k = 0; k < 3; k++)
     {

@@ -159,16 +159,20 @@ DAB_HD void revACell(const Acc& A, const Params& q, int c)
     const double pc = A.p(c), rAUc = A.rAU(c);
     const double gPc[3] = {A.gP(c, 0), A.gP(c, 1), A.gP(c, 2)};
     DAB_ACC_FACES(NF)
+    // internal faces, then boundary faces: the two passes over the row of revBCell
+    int kb = NF > 0 ? NF : A.maxCF();
     _Pragma("unroll") for (int k = 0; k < (NF > 0 ? NF : A.maxCF()); k++)
     {
         const FaceRef fr = DAB_ACC_FACE(NF, k);
-        if (fr.f < 0) break;
-        const int f = fr.f;
-        // ---- load block: everything either branch reads, issued back to back with no control flow in between (a boundary face
-        // "neighbour" is the cell itself: valid addresses, values unused).  The kernels are latency-bound; what limits them is
-        // how many loads a thread has in flight, and a branch (or the slow-path CALL of an fp64 division) ends the region the
-        // scheduler can batch loads in.
-        const int n = fr.bnd ? c : fr.n;
+        if (fr.f < 0 || fr.bnd)
+        {
+            kb = k;
+            break;
+        }
+        const int f = fr.f, n = fr.n;
+        // ---- load block: the face and the neighbour, issued back to back with no control flow in between.  The kernels are
+        // latency-bound; what limits them is how many loads a thread has in flight, and a branch (or the slow-path CALL of an
+        // fp64 division) ends the region the scheduler can batch loads in.
         const double mS = A.magSf(f), dl = A.delta(f), xphif = A.xphi(f), w = A.w(f);
         double Sv[3], kv[3];
         A.Sf(f, Sv);
@@ -177,49 +181,54 @@ DAB_HD void revACell(const Acc& A, const Params& q, int c)
         const double gPn[3] = {A.gP(n, 0), A.gP(n, 1), A.gP(n, 2)};
         const double rmS = frcp(mS);
         const double cphi = q.nrPhi ? rmS : 1.0;
-        if (!fr.bnd)
+        const double psiPn = xpn * (q.nrP ? frcp(Vn) : 1.0);
+        // F_f enters pRes_own with -1, pRes_nei with +1, phiRes_f with +1
+        const double Fb = cphi * xphif - fr.s * (psiPc - psiPn);
+        const double wc = fr.s > 0 ? w : 1.0 - w, wn = 1.0 - wc;
+        double cg = 0.0;
+        for (int j = 0; j < 3; j++) cg += kv[j] * (wc * gPc[j] + wn * gPn[j]);
+        const double sn = fr.s * dl * (pn - pc) + cg; // delta*(p_N - p_P) + corr
+        const double gam = wc * rAUc + wn * rAUn;
+        for (int j = 0; j < 3; j++)
         {
-            const double psiPn = xpn * (q.nrP ? frcp(Vn) : 1.0);
-            // F_f enters pRes_own with -1, pRes_nei with +1, phiRes_f with +1
-            const double Fb = cphi * xphif - fr.s * (psiPc - psiPn);
-            const double wc = fr.s > 0 ? w : 1.0 - w, wn = 1.0 - wc;
-            double cg = 0.0;
-            for (int j = 0; j < 3; j++) cg += kv[j] * (wc * gPc[j] + wn * gPn[j]);
-            const double sn = fr.s * dl * (pn - pc) + cg; // delta*(p_N - p_P) + corr
-            const double gam = wc * rAUc + wn * rAUn;
-            for (int j = 0; j < 3; j++)
-            {
-                HbA[j] += wc * Sv[j] * Fb;
-                gPb[j] -= gam * mS * wc * kv[j] * Fb;
-            }
-            rAUb -= wc * mS * sn * Fb;
-            pb += fr.s * gam * mS * dl * Fb;
+            HbA[j] += wc * Sv[j] * Fb;
+            gPb[j] -= gam * mS * wc * kv[j] * Fb;
+        }
+        rAUb -= wc * mS * sn * Fb;
+        pb += fr.s * gam * mS * dl * Fb;
+    }
+    _Pragma("unroll") for (int k = 0; k < (NF > 0 ? NF : A.maxCF()); k++)
+    {
+        if (k < kb) continue;
+        const FaceRef fr = DAB_ACC_FACE(NF, k);
+        if (fr.f < 0) break;
+        const int f = fr.f;
+        const double mS = A.magSf(f), dl = A.delta(f), xphif = A.xphi(f), phib = A.phi(f);
+        double Sv[3];
+        A.Sf(f, Sv);
+        const int pa = A.patch(f);
+        const double rmS = frcp(mS);
+        const double cphi = q.nrPhi ? rmS : 1.0;
+        const double Fb = cphi * xphif - psiPc;
+        const int kU = q.bcKind[F_U][pa];
+        const bool assignable = (kU == BC_INLET_OUTLET || kU == BC_OUTLET_INLET || kU == BC_ZERO_GRADIENT);
+        if (A.m.mrfType && A.m.mrfType[f - A.nIF()] == 1)
+            ; // rotating wall of the MRF zone: the relative phiHbyA is identically zero
+        else if (q.constrainHbyA && !assignable)
+        {
+            const double nh[3] = {Sv[0] * rmS, Sv[1] * rmS, Sv[2] * rmS};
+            const double valb[3] = {Sv[0] * Fb, Sv[1] * Fb, Sv[2] * Fb};
+            const double sngb[3] = {0.0, 0.0, 0.0};
+            bcVectorAdj(kU, phib, dl, nh, valb, sngb, Ub);
+            if (A.bcRefOn(pa)) bcVectorRefAdj(kU, phib, dl, valb, sngb, refb);
         }
         else
-        {
-            const int pa = A.patch(f);
-            const double phib = A.phi(f);
-            const double Fb = cphi * xphif - psiPc;
-            const int kU = q.bcKind[F_U][pa];
-            const bool assignable = (kU == BC_INLET_OUTLET || kU == BC_OUTLET_INLET || kU == BC_ZERO_GRADIENT);
-            if (A.m.mrfType && A.m.mrfType[f - A.nIF()] == 1)
-                ; // rotating wall of the MRF zone: the relative phiHbyA is identically zero
-            else if (q.constrainHbyA && !assignable)
-            {
-                const double nh[3] = {Sv[0] * rmS, Sv[1] * rmS, Sv[2] * rmS};
-                const double valb[3] = {Sv[0] * Fb, Sv[1] * Fb, Sv[2] * Fb};
-                const double sngb[3] = {0.0, 0.0, 0.0};
-                bcVectorAdj(kU, phib, dl, nh, valb, sngb, Ub);
-                if (A.bcRefOn(pa)) bcVectorRefAdj(kU, phib, dl, valb, sngb, refb);
-            }
-            else
-                for (int j = 0; j < 3; j++) HbA[j] += Sv[j] * Fb;
-            double pv, sn, frp;
-            bcScalar(q.bcKind[F_P][pa], q.bcVal[F_P][pa][0], pc, phib, dl, pv, sn, frp);
-            rAUb -= mS * sn * Fb;
-            const double snb = -rAUc * mS * Fb;
-            pb -= frp * dl * snb;
-        }
+            for (int j = 0; j < 3; j++) HbA[j] += Sv[j] * Fb;
+        double pv, sn, frp;
+        bcScalar(q.bcKind[F_P][pa], q.bcVal[F_P][pa][0], pc, phib, dl, pv, sn, frp);
+        rAUb -= mS * sn * Fb;
+        const double snb = -rAUc * mS * Fb;
+        pb -= frp * dl * snb;
     }
     // cell-level adjoint of the momentum row: URes = cU*(M + grad p), HbyA = U - rAU*M, rAU = V/(Dn + icAvg)
     const double rAU = rAUc;
@@ -271,49 +280,58 @@ struct RevA
     }
 };
 
+// The scalars of the adjoint of a cell's relaxed momentum diagonal that RevB needs, from RevA's Dn and the record's relaxation
+// flag: D1 through the active max(|D1|, sumOff) branch, so through the off-diagonal sum, D0 in total
+DAB_HD void diagAdj(double Dn, double fl, double rAl, const double* mt, const double* U, double& D1, double& so, double& D0)
+{
+    const double D2 = Dn * rAl;
+    D1 = fl != 0.0 ? fl * D2 : 0.0;
+    so = fl != 0.0 ? 0.0 : D2;
+    D0 = D1 + mt[0] * U[0] + mt[1] * U[1] + mt[2] * U[2];
+}
+
 // RevB of one cell.  FEAT: bit 0 = linearUpwindV limiter compiled in, bit 1 = wall-function nut BC compiled in, bit 2 = adjoint of
 // the boundary reference values (patchVelocity input) compiled in (the common configuration without them keeps its register
 // budget).  gradOnly (tile kernels, halo ring): only the adjoints of grad(U) / grad(nuTilda) are stored.
+//
+// A cell's ELL row lists its internal faces before its boundary faces (HostMesh::checkEllOrder), so the face loop is two passes
+// over the row: the internal pass gathers the neighbour's record with every face, the boundary pass reads only the face and the
+// cell itself.  The slots are visited in row order either way: the accumulation order is that of one loop.  Cell values that
+// are cheap to re-read (centre, volume, wall distance, grad nuTilda: L1 hits) or to recompute (trace of grad U, the SA
+// diffusivity, the diagonal scalars) are not held across the faces, so that the internal pass's load block stays in registers.
 template <int NF, int FEAT, class Acc>
 DAB_HD void revBCell(const Acc& A, const Params& q, int c, bool gradOnly)
 {
     const int schU = q.divU, schN = q.divNut;
     const double Uc[3] = {A.U(c, 0), A.U(c, 1), A.U(c, 2)};
-    const double nutc = A.nut(c);
-    const double nuEc = nutc + q.nu;
-    double gUc[9], gNc[3];
+    const double nuEc = A.nut(c) + q.nu;
+    double gUc[9];
     for (int i = 0; i < 9; i++) gUc[i] = A.gU(c, i);
     const double ntc = q.turb ? A.nt(c) : 0.0;
     const double rsig = 1.0 / SA::sigma, rAl = frcp(q.alphaU); // one division per cell instead of one per face
-    const double Gc = (ntc + q.nu) * rsig;
-    for (int i = 0; i < 3; i++) gNc[i] = q.turb ? A.gNt(c, i) : 0.0;
-    const double trc = gUc[0] + gUc[4] + gUc[8];
-    const double V = A.V(c);
-    const double Cc[3] = {A.C(c, 0), A.C(c, 1), A.C(c, 2)};
     // cell-level adjoints of row c
     const double mtc[3] = {A.mt(c, 0), A.mt(c, 1), A.mt(c, 2)};
     const double Dnc = A.Dn(c), flc = A.flag(c);
-    const double D2c = Dnc * rAl;
-    const double D1c = flc != 0.0 ? flc * D2c : 0.0;
-    const double soc = flc != 0.0 ? 0.0 : D2c;
-    const double D0c = D1c + mtc[0] * Uc[0] + mtc[1] * Uc[1] + mtc[2] * Uc[2];
-    const double psiN = q.turb ? A.xnt(c) : 0.0;
-    const double qc = psiN * (q.nrNut ? frcp(V) : 1.0); // adjoint of NV
-    const double zc = psiN * (q.nrNut ? 1.0 : V);       // adjoint of the cell-local SA sources
+    const double qc = (q.turb ? A.xnt(c) : 0.0) * (q.nrNut ? frcp(A.V(c)) : 1.0); // adjoint of NV
 
     double U2[3] = {0, 0, 0}, nt2 = 0.0, nuEb = 0.0, gUb[9], gNb[3] = {0, 0, 0};
     double refb[3] = {0, 0, 0};
     for (int i = 0; i < 9; i++) gUb[i] = 0.0;
 
     DAB_ACC_FACES(NF)
+    // ---- internal pass: slots [0, kb)
+    int kb = NF > 0 ? NF : A.maxCF();
     _Pragma("unroll") for (int k = 0; k < (NF > 0 ? NF : A.maxCF()); k++)
     {
         const FaceRef fr = DAB_ACC_FACE(NF, k);
-        if (fr.f < 0) break;
-        const int f = fr.f;
+        if (fr.f < 0 || fr.bnd)
+        {
+            kb = k;
+            break;
+        }
+        const int f = fr.f, n = fr.n;
         // ---- load block (see revACell): the face's geometry and flux and the neighbour's record, issued with no control flow in
-        // between; a boundary face reads the cell itself in place of a neighbour (valid addresses, values unused)
-        const int n = fr.bnd ? c : fr.n;
+        // between
         const double phi = A.phi(f), xphif = A.xphi(f);
         double Sv[3], kv[3], Cfv[3];
         A.Sf(f, Sv);
@@ -328,232 +346,257 @@ DAB_HD void revBCell(const Acc& A, const Params& q, int c, bool gradOnly)
         for (int i = 0; i < 9; i++) gUn[i] = A.gU(n, i);
         const double ntn = q.turb ? A.nt(n) : 0.0, xntn = q.turb ? A.xnt(n) : 0.0;
         for (int i = 0; i < 3; i++) gNn[i] = q.turb ? A.gNt(n, i) : 0.0;
+        const double Cc[3] = {A.C(c, 0), A.C(c, 1), A.C(c, 2)};
+        double gNc[3];
+        for (int i = 0; i < 3; i++) gNc[i] = q.turb ? A.gNt(c, i) : 0.0;
         const double mf = fr.s * phi;
         const double rmS = frcp(mS);
         double phib_acc = 0.0; // adjoint of phi_f (only meaningful on the owner side)
-        if (!fr.bnd)
+        const double wc = fr.s > 0 ? wf : 1.0 - wf, wn = 1.0 - wc;
+        const bool pos0 = phi >= 0.0;
+        const double wupc = fr.s > 0 ? (pos0 ? 1.0 : 0.0) : (pos0 ? 0.0 : 1.0);
+        const double nuEn = nutn + q.nu;
+        double D1c, soc, D0c, D1n, son, D0n;
+        diagAdj(Dnc, flc, rAl, mtc, Uc, D1c, soc, D0c);
+        diagAdj(Dnn, fln, rAl, mtn, Un, D1n, son, D0n);
+        const bool ownUp = phi > 0.0;
+        const bool cUp = fr.s > 0 ? ownUp : !ownUp;
+        const double dC[3] = {Cfv[0] - Cc[0], Cfv[1] - Cc[1], Cfv[2] - Cc[2]};
+        // ---- momentum rows c and n
         {
-            const double wc = fr.s > 0 ? wf : 1.0 - wf, wn = 1.0 - wc;
-            const bool pos0 = phi >= 0.0;
-            const double wupc = fr.s > 0 ? (pos0 ? 1.0 : 0.0) : (pos0 ? 0.0 : 1.0);
-            const double nuEn = nutn + q.nu;
-            const double D2n = Dnn * rAl;
-            const double D1n = fln != 0.0 ? fln * D2n : 0.0;
-            const double son = fln != 0.0 ? 0.0 : D2n;
-            const double D0n = D1n + mtn[0] * Un[0] + mtn[1] * Un[1] + mtn[2] * Un[2];
-            const bool ownUp = phi > 0.0;
-            const bool cUp = fr.s > 0 ? ownUp : !ownUp;
-            const double dC[3] = {Cfv[0] - Cc[0], Cfv[1] - Cc[1], Cfv[2] - Cc[2]};
-            // ---- momentum rows c and n
+            const double wpc = schU == DIV_LINEAR ? wc : wupc;
+            const double wpn = schU == DIV_LINEAR ? wn : 1.0 - wupc;
+            const double gf = (wc * nuEc + wn * nuEn) * mS;
+            const double g = gf * dl;
+            const double offc = mf - wpc * mf - g;
+            const double offn = -mf + wpn * mf - g;
+            const double offbc = mtc[0] * Un[0] + mtc[1] * Un[1] + mtc[2] * Un[2] + sgn(offc) * soc;
+            const double offbn = mtn[0] * Uc[0] + mtn[1] * Uc[1] + mtn[2] * Uc[2] + sgn(offn) * son;
+            for (int j = 0; j < 3; j++) U2[j] += offn * mtn[j];
+            const double abc = D0c - offbc, abn = D0n - offbn;
+            double gb = abc + abn;   // adjoint of g
+            double gfb = 0.0;        // adjoint of gf (non-orthogonal correction)
+            const double lam[3] = {fr.s * (mtc[0] - mtn[0]), fr.s * (mtc[1] - mtn[1]), fr.s * (mtc[2] - mtn[2])};
+            if (fr.s > 0)
             {
-                const double wpc = schU == DIV_LINEAR ? wc : wupc;
-                const double wpn = schU == DIV_LINEAR ? wn : 1.0 - wupc;
-                const double gf = (wc * nuEc + wn * nuEn) * mS;
-                const double g = gf * dl;
-                const double offc = mf - wpc * mf - g;
-                const double offn = -mf + wpn * mf - g;
-                const double offbc = mtc[0] * Un[0] + mtc[1] * Un[1] + mtc[2] * Un[2] + sgn(offc) * soc;
-                const double offbn = mtn[0] * Uc[0] + mtn[1] * Uc[1] + mtn[2] * Uc[2] + sgn(offn) * son;
-                for (int j = 0; j < 3; j++) U2[j] += offn * mtn[j];
-                const double abc = D0c - offbc, abn = D0n - offbn;
-                double gb = abc + abn;   // adjoint of g
-                double gfb = 0.0;        // adjoint of gf (non-orthogonal correction)
-                const double lam[3] = {fr.s * (mtc[0] - mtn[0]), fr.s * (mtc[1] - mtn[1]), fr.s * (mtc[2] - mtn[2])};
-                if (fr.s > 0)
+                const double mbc = -D0c + offbc + wpc * abc;
+                const double mbn = -D0n + offbn + wpn * abn;
+                phib_acc += mbc - mbn;
+            }
+            if (!(FEAT & 1))
+            {
+                // plain linearUpwind (compact form: no limiter state)
+                if (schU == DIV_LINEAR_UPWIND)
                 {
-                    const double mbc = -D0c + offbc + wpc * abc;
-                    const double mbn = -D0n + offbn + wpn * abn;
-                    phib_acc += mbc - mbn;
-                }
-                if (!(FEAT & 1))
-                {
-                    // plain linearUpwind (compact form: no limiter state)
-                    if (schU == DIV_LINEAR_UPWIND)
+                    if (cUp)
+                        for (int j = 0; j < 3; j++)
+                            for (int i = 0; i < 3; i++) gUb[j * 3 + i] += dC[i] * phi * lam[j];
+                    if (fr.s > 0)
                     {
-                        if (cUp)
-                            for (int j = 0; j < 3; j++)
-                                for (int i = 0; i < 3; i++) gUb[j * 3 + i] += dC[i] * phi * lam[j];
-                        if (fr.s > 0)
+                        // per-element selects: a pointer into either gradient array would put both in local memory
+                        double d[3];
+                        for (int i = 0; i < 3; i++) d[i] = cUp ? dC[i] : Cfv[i] - Cn[i];
+                        for (int j = 0; j < 3; j++)
                         {
-                            const double* gu = cUp ? gUc : gUn;
-                            double d[3];
-                            for (int i = 0; i < 3; i++) d[i] = cUp ? dC[i] : Cfv[i] - Cn[i];
-                            for (int j = 0; j < 3; j++)
-                                phib_acc += (d[0] * gu[j * 3 + 0] + d[1] * gu[j * 3 + 1] + d[2] * gu[j * 3 + 2]) * lam[j];
+                            const double gu0 = cUp ? gUc[j * 3 + 0] : gUn[j * 3 + 0], gu1 = cUp ? gUc[j * 3 + 1] : gUn[j * 3 + 1],
+                                         gu2 = cUp ? gUc[j * 3 + 2] : gUn[j * 3 + 2];
+                            phib_acc += (d[0] * gu0 + d[1] * gu1 + d[2] * gu2) * lam[j];
                         }
                     }
                 }
-                else if (schU == DIV_LINEAR_UPWIND || schU == DIV_LINEAR_UPWIND_V)
+            }
+            else if (schU == DIV_LINEAR_UPWIND || schU == DIV_LINEAR_UPWIND_V)
+            {
+                double gu[9]; // per-element selects: a pointer into either array would put both in local memory
+                for (int i = 0; i < 9; i++) gu[i] = cUp ? gUc[i] : gUn[i];
+                double d[3];
+                for (int i = 0; i < 3; i++) d[i] = cUp ? dC[i] : Cfv[i] - Cn[i];
+                double corr[3], corrL[3], outb[3], corrb[3] = {0, 0, 0};
+                for (int j = 0; j < 3; j++)
                 {
-                    const double* gu = cUp ? gUc : gUn;
-                    double d[3];
-                    for (int i = 0; i < 3; i++) d[i] = cUp ? dC[i] : Cfv[i] - Cn[i];
-                    double corr[3], corrL[3], outb[3], corrb[3] = {0, 0, 0};
+                    corr[j] = d[0] * gu[j * 3 + 0] + d[1] * gu[j * 3 + 1] + d[2] * gu[j * 3 + 2];
+                    outb[j] = phi * lam[j]; // adjoint of the (limited) correction: +phi*corr into own row, -phi*corr into nei row
+                }
+                if ((FEAT & 1) && schU == DIV_LINEAR_UPWIND_V)
+                {
+                    const double cf = ownUp ? (1.0 - wf) : -wf;
+                    double maxCorr[3], maxCorrb[3] = {0, 0, 0};
+                    for (int j = 0; j < 3; j++) maxCorr[j] = cf * fr.s * (Un[j] - Uc[j]);
+                    luvLimit(corr, maxCorr, corrL);
+                    luvLimitAdj(corr, maxCorr, outb, corrb, maxCorrb);
+                    for (int j = 0; j < 3; j++) U2[j] -= cf * fr.s * maxCorrb[j];
+                }
+                else
+                    for (int j = 0; j < 3; j++) { corrL[j] = corr[j]; corrb[j] = outb[j]; }
+                if (cUp)
                     for (int j = 0; j < 3; j++)
-                    {
-                        corr[j] = d[0] * gu[j * 3 + 0] + d[1] * gu[j * 3 + 1] + d[2] * gu[j * 3 + 2];
-                        outb[j] = phi * lam[j]; // adjoint of the (limited) correction: +phi*corr into own row, -phi*corr into nei row
-                    }
-                    if ((FEAT & 1) && schU == DIV_LINEAR_UPWIND_V)
-                    {
-                        const double cf = ownUp ? (1.0 - wf) : -wf;
-                        double maxCorr[3], maxCorrb[3] = {0, 0, 0};
-                        for (int j = 0; j < 3; j++) maxCorr[j] = cf * fr.s * (Un[j] - Uc[j]);
-                        luvLimit(corr, maxCorr, corrL);
-                        luvLimitAdj(corr, maxCorr, outb, corrb, maxCorrb);
-                        for (int j = 0; j < 3; j++) U2[j] -= cf * fr.s * maxCorrb[j];
-                    }
-                    else
-                        for (int j = 0; j < 3; j++) { corrL[j] = corr[j]; corrb[j] = outb[j]; }
-                    if (cUp)
-                        for (int j = 0; j < 3; j++)
-                            for (int i = 0; i < 3; i++) gUb[j * 3 + i] += dC[i] * corrb[j];
-                    if (fr.s > 0)
-                        for (int j = 0; j < 3; j++) phib_acc += corrL[j] * lam[j];
-                }
-                // non-orthogonal correction: MV_own -= gf*cg_j, MV_nei += gf*cg_j
-                for (int j = 0; j < 3; j++)
-                {
-                    double cg = 0.0;
-                    for (int i = 0; i < 3; i++) cg += kv[i] * (wc * gUc[j * 3 + i] + wn * gUn[j * 3 + i]);
-                    gfb -= cg * lam[j];
-                    const double cgb = -gf * lam[j];
-                    for (int i = 0; i < 3; i++) gUb[j * 3 + i] += wc * kv[i] * cgb;
-                }
-                // dev2 term: MV_own -= fl_j, MV_nei += fl_j, fl = wc*tc + wn*tn
-                double trb = 0.0;
-                for (int j = 0; j < 3; j++)
-                {
-                    const double tcb = -wc * lam[j];
-                    const double tcj = Sv[0] * gUc[0 * 3 + j] + Sv[1] * gUc[1 * 3 + j] + Sv[2] * gUc[2 * 3 + j] - (2.0 / 3.0) * trc * Sv[j];
-                    nuEb += tcb * tcj;
-                    for (int i = 0; i < 3; i++) gUb[i * 3 + j] += nuEc * Sv[i] * tcb;
-                    trb -= (2.0 / 3.0) * nuEc * Sv[j] * tcb;
-                }
-                gUb[0] += trb; gUb[4] += trb; gUb[8] += trb;
-                nuEb += wc * mS * (dl * gb + gfb);
+                        for (int i = 0; i < 3; i++) gUb[j * 3 + i] += dC[i] * corrb[j];
+                if (fr.s > 0)
+                    for (int j = 0; j < 3; j++) phib_acc += corrL[j] * lam[j];
             }
-            // ---- SA rows c and n
-            if (q.turb)
+            // non-orthogonal correction: MV_own -= gf*cg_j, MV_nei += gf*cg_j
+            for (int j = 0; j < 3; j++)
             {
-                const double qn = xntn * (q.nrNut ? frcp(Vn) : 1.0);
-                const double wpc = schN == DIV_LINEAR ? wc : wupc;
-                const double wpn = schN == DIV_LINEAR ? wn : 1.0 - wupc;
-                const double gf = (wc * Gc + wn * (ntn + q.nu) * rsig) * mS;
-                const double g = gf * dl;
-                nt2 += qc * (wpc * mf + g - mf) + qn * (-mf + wpn * mf - g);
-                const double gb = (qc - qn) * (ntc - ntn);
-                double gfb = 0.0;
-                const double lam = fr.s * (qc - qn);
-                if (fr.s > 0) phib_acc += qc * (1.0 - wpc) * (ntn - ntc) - qn * (1.0 - wpn) * (ntc - ntn);
-                if (schN == DIV_LINEAR_UPWIND)
-                {
-                    if (cUp)
-                        for (int i = 0; i < 3; i++) gNb[i] += dC[i] * phi * lam;
-                    if (fr.s > 0)
-                    {
-                        double corr = 0.0;
-                        for (int i = 0; i < 3; i++) corr += (cUp ? dC[i] * gNc[i] : (Cfv[i] - Cn[i]) * gNn[i]);
-                        phib_acc += corr * lam;
-                    }
-                }
                 double cg = 0.0;
-                for (int i = 0; i < 3; i++) cg += kv[i] * (wc * gNc[i] + wn * gNn[i]);
-                gfb -= cg * lam;
-                const double cgb = -gf * lam;
-                for (int i = 0; i < 3; i++) gNb[i] += wc * kv[i] * cgb;
-                nt2 += wc * mS * (dl * gb + gfb) * rsig;
+                for (int i = 0; i < 3; i++) cg += kv[i] * (wc * gUc[j * 3 + i] + wn * gUn[j * 3 + i]);
+                gfb -= cg * lam[j];
+                const double cgb = -gf * lam[j];
+                for (int i = 0; i < 3; i++) gUb[j * 3 + i] += wc * kv[i] * cgb;
             }
-        }
-        else
-        {
-            const int pa = A.patch(f);
-            const double nh[3] = {Sv[0] * rmS, Sv[1] * rmS, Sv[2] * rmS};
-            const int kU = q.bcKind[F_U][pa];
-            BCv bu;
-            double uw[3];
-            mrfWallRef(A.m, f, q.bcVal[F_U][pa], uw);
-            bcVector(kU, uw, Uc, mf, dl, nh, bu);
-            double ntb = 0.0, sngN = 0.0, frN = 0.0;
-            if (q.turb) bcScalar(q.bcKind[F_NUTILDA][pa], q.bcVal[F_NUTILDA][pa][0], ntc, mf, dl, ntb, sngN, frN);
-            double dP = 0.0, dNb = 0.0, dUn[3] = {0.0, 0.0, 0.0};
-            double nutb = 0.0;
-            if (q.turb)
-                nutb = (FEAT & 2) ? nutBoundary<true>(q.bcKind[F_NUT][pa], q.bcVal[F_NUT][pa][0], nutc, ntb, q.nu, Uc, bu.val, dl, dP, dNb, dUn)
-                                  : nutBoundaryBasic(q.bcKind[F_NUT][pa], q.bcVal[F_NUT][pa][0], nutc, ntb, q.nu, dP, dNb);
-            const double nuEB = nutb + q.nu;
-            const double G = nuEB * mS;
-            // internalCoeffs and the argmax/argmin components used by relax()
-            double ic[3];
-            int kmax = 0, kmin = 0;
+            // dev2 term: MV_own -= fl_j, MV_nei += fl_j, fl = wc*tc + wn*tn
+            const double trc = gUc[0] + gUc[4] + gUc[8];
+            double trb = 0.0;
             for (int j = 0; j < 3; j++)
             {
-                ic[j] = mf * bu.vic[j] - G * bu.gic[j];
-                if (j > 0)
+                const double tcb = -wc * lam[j];
+                const double tcj = Sv[0] * gUc[0 * 3 + j] + Sv[1] * gUc[1 * 3 + j] + Sv[2] * gUc[2 * 3 + j] - (2.0 / 3.0) * trc * Sv[j];
+                nuEb += tcb * tcj;
+                for (int i = 0; i < 3; i++) gUb[i * 3 + j] += nuEc * Sv[i] * tcb;
+                trb -= (2.0 / 3.0) * nuEc * Sv[j] * tcb;
+            }
+            gUb[0] += trb; gUb[4] += trb; gUb[8] += trb;
+            nuEb += wc * mS * (dl * gb + gfb);
+        }
+        // ---- SA rows c and n
+        if (q.turb)
+        {
+            const double qn = xntn * (q.nrNut ? frcp(Vn) : 1.0);
+            const double wpc = schN == DIV_LINEAR ? wc : wupc;
+            const double wpn = schN == DIV_LINEAR ? wn : 1.0 - wupc;
+            const double Gc = (ntc + q.nu) * rsig;
+            const double gf = (wc * Gc + wn * (ntn + q.nu) * rsig) * mS;
+            const double g = gf * dl;
+            nt2 += qc * (wpc * mf + g - mf) + qn * (-mf + wpn * mf - g);
+            const double gb = (qc - qn) * (ntc - ntn);
+            double gfb = 0.0;
+            const double lam = fr.s * (qc - qn);
+            if (fr.s > 0) phib_acc += qc * (1.0 - wpc) * (ntn - ntc) - qn * (1.0 - wpn) * (ntc - ntn);
+            if (schN == DIV_LINEAR_UPWIND)
+            {
+                if (cUp)
+                    for (int i = 0; i < 3; i++) gNb[i] += dC[i] * phi * lam;
+                if (fr.s > 0)
                 {
-                    if (fabs(ic[j]) > fabs(ic[kmax])) kmax = j;
-                    if (ic[j] < ic[kmin]) kmin = j;
+                    double corr = 0.0;
+                    for (int i = 0; i < 3; i++) corr += (cUp ? dC[i] * gNc[i] : (Cfv[i] - Cn[i]) * gNn[i]);
+                    phib_acc += corr * lam;
                 }
             }
-            double mb = -D0c, Gb_ = 0.0;
-            for (int j = 0; j < 3; j++)
-            {
-                double icb = Dnc * (1.0 / 3.0);
-                if (j == kmin) icb -= Dnc;
-                if (j == kmax) icb += D1c * sgn(ic[j]);
-                mb += bu.vic[j] * icb + mtc[j] * bu.val[j];
-                Gb_ += -bu.gic[j] * icb - mtc[j] * bu.sng[j];
-            }
-            double valb[3], sngb[3];
-            for (int j = 0; j < 3; j++) { valb[j] = mf * mtc[j]; sngb[j] = -G * mtc[j]; }
-            // dev2 boundary term: MV_j -= nuEB * X_j
-            double Gbd[9];
-            for (int j = 0; j < 3; j++)
-            {
-                const double nG = nh[0] * gUc[j * 3 + 0] + nh[1] * gUc[j * 3 + 1] + nh[2] * gUc[j * 3 + 2];
-                for (int i = 0; i < 3; i++) Gbd[j * 3 + i] = gUc[j * 3 + i] + nh[i] * (bu.sng[j] - nG);
-            }
-            const double trbv = Gbd[0] + Gbd[4] + Gbd[8];
-            double nuEBb = mS * Gb_;
-            double Gbb[9];
-            for (int i = 0; i < 9; i++) Gbb[i] = 0.0;
-            double trbb = 0.0;
-            for (int j = 0; j < 3; j++)
-            {
-                const double X = Sv[0] * Gbd[0 * 3 + j] + Sv[1] * Gbd[1 * 3 + j] + Sv[2] * Gbd[2 * 3 + j] - (2.0 / 3.0) * trbv * Sv[j];
-                nuEBb -= X * mtc[j];
-                const double Xb = -nuEB * mtc[j];
-                for (int i = 0; i < 3; i++) Gbb[i * 3 + j] += Sv[i] * Xb;
-                trbb -= (2.0 / 3.0) * Sv[j] * Xb;
-            }
-            Gbb[0] += trbb; Gbb[4] += trbb; Gbb[8] += trbb;
-            boundaryGradAdj(nh, Gbb, gUb, sngb);
-            bcVectorAdj(kU, mf, dl, nh, valb, sngb, U2);
-            if ((FEAT & 4) && A.bcRefOn(pa)) bcVectorRefAdj(kU, mf, dl, valb, sngb, refb);
-            // nut_b -> nut_c / nuTilda_b / U_c (wall function)
-            nuEb += dP * nuEBb;
-            if (FEAT & 2)
-                for (int j = 0; j < 3; j++) U2[j] += dUn[j] * nuEBb;
-            double ntbb = dNb * nuEBb;
-            if (q.turb)
-            {
-                const double Gs = (ntb + q.nu) * rsig * mS;
-                mb += qc * (ntb - ntc);
-                ntbb += qc * mf - qc * sngN * mS * rsig;
-                const double sngNb = -qc * Gs;
-                nt2 += -qc * mf + (1.0 - frN) * ntbb - frN * dl * sngNb;
-            }
-            phib_acc += mb;
+            double cg = 0.0;
+            for (int i = 0; i < 3; i++) cg += kv[i] * (wc * gNc[i] + wn * gNn[i]);
+            gfb -= cg * lam;
+            const double cgb = -gf * lam;
+            for (int i = 0; i < 3; i++) gNb[i] += wc * kv[i] * cgb;
+            nt2 += wc * mS * (dl * gb + gfb) * rsig;
         }
         if (!gradOnly)
         {
             if (fr.s > 0)
                 A.setYPhi(f, (phib_acc - (q.nrPhi ? rmS : 1.0) * xphif) * phiRowScale(q, mS));
-            else if (A.ghost(fr.n))
+            else if (A.ghost(n))
                 A.setYPhi(f, 0.0); // cut face whose phi belongs to the neighbouring rank
         }
     }
-    if (q.turb) saSourceAdj(ntc, q.nu, A.yWall(c), gUc, gNc, zc, nt2, gUb, gNb, q.saFv3);
+    // ---- boundary pass: slots [kb, maxCF) are boundary faces (the cell is their owner) up to the first padding slot
+    _Pragma("unroll") for (int k = 0; k < (NF > 0 ? NF : A.maxCF()); k++)
+    {
+        if (k < kb) continue;
+        const FaceRef fr = DAB_ACC_FACE(NF, k);
+        if (fr.f < 0) break;
+        const int f = fr.f;
+        const double phi = A.phi(f), xphif = A.xphi(f);
+        double Sv[3];
+        A.Sf(f, Sv);
+        const double mS = A.magSf(f), dl = A.delta(f);
+        const int pa = A.patch(f);
+        const double nutc = A.nut(c);
+        const double mf = phi; // outward flux: s = +1
+        const double rmS = frcp(mS);
+        double D1c, soc, D0c;
+        diagAdj(Dnc, flc, rAl, mtc, Uc, D1c, soc, D0c);
+        const double nh[3] = {Sv[0] * rmS, Sv[1] * rmS, Sv[2] * rmS};
+        const int kU = q.bcKind[F_U][pa];
+        BCv bu;
+        double uw[3];
+        mrfWallRef(A.m, f, q.bcVal[F_U][pa], uw);
+        bcVector(kU, uw, Uc, mf, dl, nh, bu);
+        double ntb = 0.0, sngN = 0.0, frN = 0.0;
+        if (q.turb) bcScalar(q.bcKind[F_NUTILDA][pa], q.bcVal[F_NUTILDA][pa][0], ntc, mf, dl, ntb, sngN, frN);
+        double dP = 0.0, dNb = 0.0, dUn[3] = {0.0, 0.0, 0.0};
+        double nutb = 0.0;
+        if (q.turb)
+            nutb = (FEAT & 2) ? nutBoundary<true>(q.bcKind[F_NUT][pa], q.bcVal[F_NUT][pa][0], nutc, ntb, q.nu, Uc, bu.val, dl, dP, dNb, dUn)
+                              : nutBoundaryBasic(q.bcKind[F_NUT][pa], q.bcVal[F_NUT][pa][0], nutc, ntb, q.nu, dP, dNb);
+        const double nuEB = nutb + q.nu;
+        const double G = nuEB * mS;
+        // internalCoeffs and the argmax/argmin components used by relax(); the extrema and the sign at the argmax are carried by
+        // value (read back through kmax / kmin, the array would live in local memory)
+        double ic[3];
+        for (int j = 0; j < 3; j++) ic[j] = mf * bu.vic[j] - G * bu.gic[j];
+        int kmax = 0, kmin = 0;
+        double icMaxAbs = fabs(ic[0]), icMin = ic[0], sgnMax = sgn(ic[0]);
+        for (int j = 1; j < 3; j++)
+        {
+            if (fabs(ic[j]) > icMaxAbs) { kmax = j; icMaxAbs = fabs(ic[j]); sgnMax = sgn(ic[j]); }
+            if (ic[j] < icMin) { kmin = j; icMin = ic[j]; }
+        }
+        double mb = -D0c, Gb_ = 0.0;
+        for (int j = 0; j < 3; j++)
+        {
+            double icb = Dnc * (1.0 / 3.0);
+            if (j == kmin) icb -= Dnc;
+            if (j == kmax) icb += D1c * sgnMax;
+            mb += bu.vic[j] * icb + mtc[j] * bu.val[j];
+            Gb_ += -bu.gic[j] * icb - mtc[j] * bu.sng[j];
+        }
+        double valb[3], sngb[3];
+        for (int j = 0; j < 3; j++) { valb[j] = mf * mtc[j]; sngb[j] = -G * mtc[j]; }
+        // dev2 boundary term: MV_j -= nuEB * X_j
+        double Gbd[9];
+        for (int j = 0; j < 3; j++)
+        {
+            const double nG = nh[0] * gUc[j * 3 + 0] + nh[1] * gUc[j * 3 + 1] + nh[2] * gUc[j * 3 + 2];
+            for (int i = 0; i < 3; i++) Gbd[j * 3 + i] = gUc[j * 3 + i] + nh[i] * (bu.sng[j] - nG);
+        }
+        const double trbv = Gbd[0] + Gbd[4] + Gbd[8];
+        double nuEBb = mS * Gb_;
+        double Gbb[9];
+        for (int i = 0; i < 9; i++) Gbb[i] = 0.0;
+        double trbb = 0.0;
+        for (int j = 0; j < 3; j++)
+        {
+            const double X = Sv[0] * Gbd[0 * 3 + j] + Sv[1] * Gbd[1 * 3 + j] + Sv[2] * Gbd[2 * 3 + j] - (2.0 / 3.0) * trbv * Sv[j];
+            nuEBb -= X * mtc[j];
+            const double Xb = -nuEB * mtc[j];
+            for (int i = 0; i < 3; i++) Gbb[i * 3 + j] += Sv[i] * Xb;
+            trbb -= (2.0 / 3.0) * Sv[j] * Xb;
+        }
+        Gbb[0] += trbb; Gbb[4] += trbb; Gbb[8] += trbb;
+        boundaryGradAdj(nh, Gbb, gUb, sngb);
+        bcVectorAdj(kU, mf, dl, nh, valb, sngb, U2);
+        if ((FEAT & 4) && A.bcRefOn(pa)) bcVectorRefAdj(kU, mf, dl, valb, sngb, refb);
+        // nut_b -> nut_c / nuTilda_b / U_c (wall function)
+        nuEb += dP * nuEBb;
+        if (FEAT & 2)
+            for (int j = 0; j < 3; j++) U2[j] += dUn[j] * nuEBb;
+        double ntbb = dNb * nuEBb;
+        if (q.turb)
+        {
+            const double Gs = (ntb + q.nu) * rsig * mS;
+            mb += qc * (ntb - ntc);
+            ntbb += qc * mf - qc * sngN * mS * rsig;
+            const double sngNb = -qc * Gs;
+            nt2 += -qc * mf + (1.0 - frN) * ntbb - frN * dl * sngNb;
+        }
+        double phib_acc = 0.0;
+        phib_acc += mb;
+        if (!gradOnly) A.setYPhi(f, (phib_acc - (q.nrPhi ? rmS : 1.0) * xphif) * phiRowScale(q, mS));
+    }
+    if (q.turb)
+    {
+        const double gNc[3] = {A.gNt(c, 0), A.gNt(c, 1), A.gNt(c, 2)};
+        saSourceAdj(ntc, q.nu, A.yWall(c), gUc, gNc, A.xnt(c) * (q.nrNut ? 1.0 : A.V(c)), nt2, gUb, gNb, q.saFv3); // zc: adjoint of the cell-local SA sources
+    }
     if (!gradOnly)
     {
         for (int j = 0; j < 3; j++) A.setU2(c, j, U2[j]);
@@ -600,13 +643,18 @@ DAB_HD void revCCell(const Acc& A, const Params& q, int c, int functionMode)
     if (q.turb) nb = A.nt2(c) + A.nutb(c) * dnut_dnt(A.nt(c), q.nu);
     double refb[3] = {0, 0, 0};
     DAB_ACC_FACES(NF)
+    // internal faces, then boundary faces: the two passes over the row of revBCell
+    int kb = NF > 0 ? NF : A.maxCF();
     _Pragma("unroll") for (int k = 0; k < (NF > 0 ? NF : A.maxCF()); k++)
     {
         const FaceRef fr = DAB_ACC_FACE(NF, k);
-        if (fr.f < 0) break;
-        const int f = fr.f;
-        // load block (see revACell): the neighbour's gradient adjoints of an internal face, the cell's own for a boundary face
-        const int n = fr.bnd ? c : fr.n;
+        if (fr.f < 0 || fr.bnd)
+        {
+            kb = k;
+            break;
+        }
+        const int f = fr.f, n = fr.n;
+        // load block (see revACell): the neighbour's gradient adjoints
         double Sv[3];
         A.Sf(f, Sv);
         const double wf = A.w(f), Vn = A.V(n);
@@ -618,43 +666,47 @@ DAB_HD void revCCell(const Acc& A, const Params& q, int c, int functionMode)
             gNbn[i] = q.turb ? A.gNtb(n, i) : 0.0;
         }
         const double So[3] = {fr.s * Sv[0], fr.s * Sv[1], fr.s * Sv[2]}; // outward
-        if (!fr.bnd)
+        const double wc = fr.s > 0 ? wf : 1.0 - wf;
+        const double iVn = frcp(Vn);
+        for (int j = 0; j < 3; j++)
         {
-            const double wc = fr.s > 0 ? wf : 1.0 - wf;
-            const double iVn = frcp(Vn);
-            for (int j = 0; j < 3; j++)
-            {
-                double t = 0.0;
-                for (int i = 0; i < 3; i++) t += So[i] * (gUbc[j * 3 + i] - gUbn[j * 3 + i] * iVn);
-                Ub[j] += wc * t;
-            }
-            double tp = 0.0, tn = 0.0;
-            for (int i = 0; i < 3; i++)
-            {
-                tp += So[i] * (gPbc[i] - gPbn[i] * iVn);
-                if (q.turb) tn += So[i] * (gNbc[i] - gNbn[i] * iVn);
-            }
-            pb += wc * tp;
-            nb += wc * tn;
+            double t = 0.0;
+            for (int i = 0; i < 3; i++) t += So[i] * (gUbc[j * 3 + i] - gUbn[j * 3 + i] * iVn);
+            Ub[j] += wc * t;
         }
-        else
+        double tp = 0.0, tn = 0.0;
+        for (int i = 0; i < 3; i++)
         {
-            const int pa = A.patch(f);
-            const double phib = A.phi(f), dl = A.delta(f);
-            const double im = frcp(A.magSf(f));
-            const double nh[3] = {Sv[0] * im, Sv[1] * im, Sv[2] * im};
-            double valb[3];
-            const double sngb[3] = {0.0, 0.0, 0.0};
-            for (int j = 0; j < 3; j++) valb[j] = So[0] * gUbc[j * 3 + 0] + So[1] * gUbc[j * 3 + 1] + So[2] * gUbc[j * 3 + 2];
-            bcVectorAdj(q.bcKind[F_U][pa], phib, dl, nh, valb, sngb, Ub);
-            if (A.bcRefOn(pa)) bcVectorRefAdj(q.bcKind[F_U][pa], phib, dl, valb, sngb, refb);
-            const double frp = bcFrac(q.bcKind[F_P][pa], phib);
-            pb += (1.0 - frp) * (So[0] * gPbc[0] + So[1] * gPbc[1] + So[2] * gPbc[2]);
-            if (q.turb)
-            {
-                const double frn = bcFrac(q.bcKind[F_NUTILDA][pa], phib);
-                nb += (1.0 - frn) * (So[0] * gNbc[0] + So[1] * gNbc[1] + So[2] * gNbc[2]);
-            }
+            tp += So[i] * (gPbc[i] - gPbn[i] * iVn);
+            if (q.turb) tn += So[i] * (gNbc[i] - gNbn[i] * iVn);
+        }
+        pb += wc * tp;
+        nb += wc * tn;
+    }
+    _Pragma("unroll") for (int k = 0; k < (NF > 0 ? NF : A.maxCF()); k++)
+    {
+        if (k < kb) continue;
+        const FaceRef fr = DAB_ACC_FACE(NF, k);
+        if (fr.f < 0) break;
+        const int f = fr.f;
+        double Sv[3];
+        A.Sf(f, Sv);
+        const double So[3] = {fr.s * Sv[0], fr.s * Sv[1], fr.s * Sv[2]}; // outward
+        const int pa = A.patch(f);
+        const double phib = A.phi(f), dl = A.delta(f);
+        const double im = frcp(A.magSf(f));
+        const double nh[3] = {Sv[0] * im, Sv[1] * im, Sv[2] * im};
+        double valb[3];
+        const double sngb[3] = {0.0, 0.0, 0.0};
+        for (int j = 0; j < 3; j++) valb[j] = So[0] * gUbc[j * 3 + 0] + So[1] * gUbc[j * 3 + 1] + So[2] * gUbc[j * 3 + 2];
+        bcVectorAdj(q.bcKind[F_U][pa], phib, dl, nh, valb, sngb, Ub);
+        if (A.bcRefOn(pa)) bcVectorRefAdj(q.bcKind[F_U][pa], phib, dl, valb, sngb, refb);
+        const double frp = bcFrac(q.bcKind[F_P][pa], phib);
+        pb += (1.0 - frp) * (So[0] * gPbc[0] + So[1] * gPbc[1] + So[2] * gPbc[2]);
+        if (q.turb)
+        {
+            const double frn = bcFrac(q.bcKind[F_NUTILDA][pa], phib);
+            nb += (1.0 - frn) * (So[0] * gNbc[0] + So[1] * gNbc[1] + So[2] * gNbc[2]);
         }
     }
     if (A.bcRefAny())

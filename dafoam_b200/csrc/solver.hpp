@@ -20,6 +20,7 @@
 #include "primal_kernels.hpp"
 #include "geom_kernels.hpp"
 #include "comp_primal_kernels.hpp"
+#include "launch_traits.hpp"
 #include "partition.hpp"
 #include "comm.hpp"
 #include <chrono>
@@ -32,45 +33,6 @@
 
 namespace dab
 {
-
-#if !defined(DAB_HOSTSIM)
-#ifndef DAB_REVB_MINBLOCKS
-#define DAB_REVB_MINBLOCKS 3
-#endif
-#ifndef DAB_FWDB_MINBLOCKS
-#define DAB_FWDB_MINBLOCKS 3
-#endif
-template <int NF, int FEAT> struct LaunchTraits<RevB<NF, FEAT>> { static constexpr int minBlocks = DAB_REVB_MINBLOCKS; };
-// with the hoisted load blocks: RevA 96 registers / 5 CTAs per SM, RevC 128 / 4
-template <int NF> struct LaunchTraits<RevA<NF>> { static constexpr int minBlocks = 5; };
-template <int NF> struct LaunchTraits<RevC<NF>> { static constexpr int minBlocks = 4; };
-template <int NF, int FEAT> struct LaunchTraits<FwdB<NF, FEAT>> { static constexpr int minBlocks = DAB_FWDB_MINBLOCKS; };
-template <int NF, int FEAT> struct LaunchTraits<UEqnAssemble<NF, FEAT>> { static constexpr int minBlocks = DAB_FWDB_MINBLOCKS; };
-template <int NF> struct LaunchTraits<NutEqnAssemble<NF>> { static constexpr int minBlocks = 4; };
-template <int NF> struct LaunchTraits<cFwdB<NF>> { static constexpr int minBlocks = 2; };
-template <int NF> struct LaunchTraits<cUEqnAssemble<NF>> { static constexpr int minBlocks = 2; };
-template <int NF> struct LaunchTraits<cEEqnAssemble<NF>> { static constexpr int minBlocks = 3; };
-template <int NF> struct LaunchTraits<cNutEqnAssemble<NF>> { static constexpr int minBlocks = 3; };
-template <int NF> struct LaunchTraits<cPEqnAssemble<NF>> { static constexpr int minBlocks = 4; };
-template <int NF> struct LaunchTraits<cPhiUpdate<NF>> { static constexpr int minBlocks = 4; };
-// resident CTAs per SM of the compressible reverse kernels: cRevA 4, cRevB 3 (168 registers, with spills), cRevE (+cRevC) 4 --
-// these kernels wait on gathers: more warps beat fewer spills
-#ifndef DAB_CREVA_MINBLOCKS
-#define DAB_CREVA_MINBLOCKS 4
-#endif
-#ifndef DAB_CREVB_MINBLOCKS
-#define DAB_CREVB_MINBLOCKS 3
-#endif
-#ifndef DAB_CREVE_MINBLOCKS
-#define DAB_CREVE_MINBLOCKS 4
-#endif
-template <int NF> struct LaunchTraits<cRevB<NF>> { static constexpr int minBlocks = DAB_CREVB_MINBLOCKS; };
-template <int NF> struct LaunchTraits<cRevA<NF>> { static constexpr int minBlocks = DAB_CREVA_MINBLOCKS; };
-template <int NF> struct LaunchTraits<cRevE<NF>> { static constexpr int minBlocks = DAB_CREVE_MINBLOCKS; };
-template <int NF> struct LaunchTraits<cRevC<NF>> { static constexpr int minBlocks = 4; };
-template <int NF> struct LaunchTraits<cFwdE<NF>> { static constexpr int minBlocks = 4; };
-template <int NF> struct LaunchTraits<cFwdC<NF>> { static constexpr int minBlocks = 4; };
-#endif
 
 // optional-feature dispatch for the two heavy kernels (hex meshes: 4 variants; other meshes: the full-featured one)
 #define DAB_LAUNCH_NFF(n, F, ...)                                     \
