@@ -451,6 +451,54 @@ int dab_get_pc_matrix(dab_solver* s, int64_t* n_rows, int64_t* nnz, int64_t* row
     DAB_CATCH
 }
 
+int dab_get_pc_factors(dab_solver* s, int64_t* n_rows, int64_t* nnz, int64_t* row_ptr, int32_t* cols, double* vals, int32_t* perm,
+                       int32_t* colour)
+{
+    DAB_TRY
+    need(s, "solver");
+    need(n_rows, "n_rows");
+    need(nnz, "nnz");
+    Solver& S = s->s;
+    if (!S.kry.pcFactored) throw Error("dab_get_pc_factors: no ILU(0) factorisation: call dab_calc_drdwt_pc first");
+    if (!row_ptr)
+    {
+        *n_rows = S.kry.n;
+        *nnz = S.kry.nnz;
+        return 0;
+    }
+    need(cols, "cols");
+    need(vals, "vals");
+    need(perm, "perm");
+    need(colour, "colour");
+    std::vector<int64_t> rp;
+    std::vector<int32_t> cl, pm, co;
+    std::vector<double> vl;
+    S.exportPCFactors(rp, cl, vl, pm, co);
+    if ((int64_t)cl.size() > *nnz || (int64_t)rp.size() - 1 > *n_rows) throw Error("dab_get_pc_factors: the buffers are too small");
+    *n_rows = (int64_t)rp.size() - 1;
+    *nnz = (int64_t)cl.size();
+    std::copy(rp.begin(), rp.end(), row_ptr);
+    std::copy(cl.begin(), cl.end(), cols);
+    std::copy(vl.begin(), vl.end(), vals);
+    std::copy(pm.begin(), pm.end(), perm);
+    std::copy(co.begin(), co.end(), colour);
+    DAB_CATCH
+}
+
+int dab_get_pc_aggregates(dab_solver* s, int32_t* agg_of)
+{
+    DAB_TRY
+    need(s, "solver");
+    need(agg_of, "agg_of");
+    Solver& S = s->s;
+    const Coarse& Cs = S.kry.coarse;
+    if (!Cs.enabled || !Cs.valid) throw Error("dab_get_pc_aggregates: the preconditioner has no coarse space (adjEqnOption.coarseAggregates)");
+    std::vector<int32_t> a((size_t)S.hm.nC);
+    S.be.d2h(a.data(), Cs.dAggOf.p, a.size() * sizeof(int32_t));
+    for (int c = 0; c < S.hm.nC; c++) agg_of[c] = Cs.aggBase + a[c];
+    DAB_CATCH
+}
+
 int dab_calc_pc_mat_fvmatrix(dab_solver* s, int turb_only, int64_t* nnz, int32_t* rows, int32_t* cols, double* vals)
 {
     DAB_TRY

@@ -2016,6 +2016,48 @@ struct Solver
         }
     }
 
+    // test hook: the ILU(0) factors of the last calcPC in factorisation order (rows and columns in the new numbering), CSR with
+    // sorted columns: L multipliers left of the diagonal, the stored 1 / u_ii on it, U right of it -- the values the triangular
+    // solves read (the fp32 copy widened with pcStorage fp32).  perm[new] = external index, colour[new] = ordering colour of the row.
+    void exportPCFactors(std::vector<int64_t>& rowPtr, std::vector<int32_t>& cols, std::vector<double>& vals, std::vector<int32_t>& perm,
+                         std::vector<int32_t>& colour)
+    {
+        Krylov& K = kry;
+        if (!K.pcFactored || K.ellSize == 0) throw Error("no ILU(0) factorisation: call calcdRdWT first");
+        std::vector<int32_t> hc((size_t)K.ellSize);
+        be.d2h(hc.data(), K.dCol.p, (size_t)K.ellSize * sizeof(int32_t));
+        std::vector<double> hv((size_t)K.ellSize);
+        if (K.useF32)
+        {
+            std::vector<float> hf((size_t)K.ellSize);
+            be.d2h(hf.data(), K.dValF.p, (size_t)K.ellSize * sizeof(float));
+            for (size_t o = 0; o < hf.size(); o++) hv[o] = (double)hf[o];
+        }
+        else
+            be.d2h(hv.data(), K.dVal.p, (size_t)K.ellSize * sizeof(double));
+        rowPtr.assign((size_t)K.n + 1, 0);
+        cols.clear();
+        vals.clear();
+        for (int i = 0; i < K.n; i++)
+        {
+            for (int q = 0; q < K.rowLen[i]; q++) // ELL rows are sorted by column
+            {
+                const size_t at = (size_t)(K.rowBase[i] + (int64_t)q * K.rowStride[i]);
+                cols.push_back(hc[at]);
+                vals.push_back(hv[at]);
+            }
+            rowPtr[(size_t)i + 1] = (int64_t)cols.size();
+        }
+        perm.assign(K.perm.begin(), K.perm.end());
+        colour.assign(K.n, -1);
+        for (size_t k = 0; k < K.colours.size(); k++)
+        {
+            const ColourView& cv = K.colours[k];
+            for (int s = 0; s < cv.nSlots; s++)
+                for (int t = 0; t < cv.slotCount[s]; t++) colour[cv.slotStart[s] + t] = (int32_t)k;
+        }
+    }
+
     // the two area averages of DAFunctionTotalPressureRatio: side 0 = outlet (numerator), 1 = inlet
     ForceSpec tprSpec(const FunctionDef& f, int side) const
     {

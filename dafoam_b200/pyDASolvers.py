@@ -582,6 +582,25 @@ class pyDASolvers:
                                               cl.ctypes.data_as(C.POINTER(C.c_int32)), _dp(vl)))
         return rp, cl[:nnz.value], vl[:nnz.value]
 
+    def getPCFactors(self):
+        """Test hook: (row_ptr, cols, vals, perm, colour) of the ILU(0) factors of the last calcdRdWT(1, ...) in factorisation order
+        (CSR, sorted columns): L multipliers left of the diagonal, the stored 1/u_ii on it, U right of it, as the triangular solves
+        read them; perm[new] = external state index, colour[new] = ordering colour of the row."""
+        n, nnz = C.c_int64(), C.c_int64()
+        self._raise(self._L.dab_get_pc_factors(self._h, C.byref(n), C.byref(nnz), None, None, None, None, None))
+        rp, cl, vl = np.zeros(n.value + 1, dtype=np.int64), np.zeros(nnz.value, dtype=np.int32), np.zeros(nnz.value)
+        perm, colour = np.zeros(n.value, dtype=np.int32), np.zeros(n.value, dtype=np.int32)
+        ip = C.POINTER(C.c_int32)
+        self._raise(self._L.dab_get_pc_factors(self._h, C.byref(n), C.byref(nnz), rp.ctypes.data_as(C.POINTER(C.c_int64)),
+                                               cl.ctypes.data_as(ip), _dp(vl), perm.ctypes.data_as(ip), colour.ctypes.data_as(ip)))
+        return rp, cl[:nnz.value], vl[:nnz.value], perm, colour
+
+    def getPCAggregates(self):
+        """Test hook: the global aggregate id of every local cell of the preconditioner's pressure coarse space."""
+        agg = np.zeros(self.getNLocalCells(), dtype=np.int32)
+        self._raise(self._L.dab_get_pc_aggregates(self._h, agg.ctypes.data_as(C.POINTER(C.c_int32))))
+        return agg
+
     def initializedRdWTMatrixFree(self):
         return None
 

@@ -189,6 +189,18 @@ int dab_run_fp_adj(dab_solver* s, const double* dfdw, double* psi, int* fail, da
  * dab_calc_drdwt_pc, otherwise only the factorisation is kept. */
 int dab_get_pc_matrix(dab_solver* s, int64_t* n_rows, int64_t* nnz, int64_t* row_ptr, int32_t* cols, double* vals);
 
+/* Test hook (no counterpart in the reference): the ILU(0) factors of the last dab_calc_drdwt_pc in factorisation order, CSR with
+ * sorted columns -- strictly lower entries are the L multipliers, the diagonal holds the stored reciprocal 1/u_ii, upper entries are
+ * U; the values the triangular solves read (the fp32 copy widened when adjEqnOption.pcStorage is "fp32").  perm[new] = external
+ * state index, colour[new] = ordering colour (level) of the row.  Same two-call size protocol as dab_get_pc_matrix; perm and colour
+ * take n_rows entries.  Does not need writeJacobians. */
+int dab_get_pc_factors(dab_solver* s, int64_t* n_rows, int64_t* nnz, int64_t* row_ptr, int32_t* cols, double* vals, int32_t* perm,
+                       int32_t* colour);
+
+/* Test hook (no counterpart in the reference): the global aggregate id of every local cell of the preconditioner's pressure coarse
+ * space (adjEqnOption.coarseAggregates > 0); an error without a coarse space. */
+int dab_get_pc_aggregates(dab_solver* s, int32_t* agg_of);
+
 /* calcPCMatWithFvMatrix(PCMat, turbOnly) (reference pyDASolvers.pyx:99-114 list, DASolver.C:2888-2988): the turbulence block of
  * the preconditioner taken from the relaxed nuTilda fvMatrix (diag / lower / upper, `div(pc)` convection, DASpalartAllmaras.C:
  * 490-529), scaled and transposed like the reference, as COO triplets (row, column, value) in the local state numbering -- what the
