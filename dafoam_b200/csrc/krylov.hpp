@@ -781,6 +781,13 @@ struct Krylov
     // GMRES workspace
     DevBuf<double> V, w, z, xdev, bdev, hdev;
     int vCap = 0;
+    // hdev <- count host coefficients.  GMRES (m + 1 per cycle) and IDR(s) (s) share the buffer on one handle, so a copy larger
+    // than it is an error rather than a write past the allocation
+    void putCoeffs(Backend& be, const double* h, int count)
+    {
+        if ((size_t)count > hdev.n) throw Error("Krylov coefficient buffer holds " + std::to_string(hdev.n) + " values, " + std::to_string(count) + " needed");
+        be.h2d(hdev.p, h, (size_t)count * sizeof(double));
+    }
     DevBuf<double> idr; // IDR(s) workspace: P(s) | G(s) | U(s) | r | t | v | z
     int idrS = 0;
     bool idrShadowReady = false;

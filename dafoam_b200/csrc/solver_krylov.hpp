@@ -946,7 +946,7 @@ inline int Solver::solveLinearEqn(const double* rhs, double* sol, KspStats& st)
         K.z.alloc(be, n);
         K.xdev.alloc(be, n);
         K.bdev.alloc(be, n);
-        K.hdev.alloc(be, m + 2);
+        if (K.hdev.n < (size_t)(m + 2)) K.hdev.alloc(be, m + 2); // grow-only: IDR(s) may keep using it with s > m + 2
         K.ops.init(be, &comm, m + 2);
     }
     be.h2d(K.bdev.p, rhs, (size_t)n * sizeof(double));
@@ -1001,7 +1001,7 @@ inline int Solver::solveLinearEqn(const double* rhs, double* sol, KspStats& st)
             const double* d = K.ops.dots(K.V.p, n, k + 2, vk1, n); // V_0..V_k . w and w . w (V_{k+1} = w)
             for (int j = 0; j <= k; j++) hcol[j] = d[j];
             const double wn2 = d[k + 1];
-            be.h2d(K.hdev.p, hcol.data(), (size_t)(k + 1) * sizeof(double));
+            K.putCoeffs(be, hcol.data(), k + 1);
             be.launch(n, MultiAxpy{K.V.p, n, k + 1, K.hdev.p, vk1, 0});
             // ||w - V h||^2 = ||w||^2 - ||h||^2 (V orthonormal); refine -- and measure the norm explicitly -- only when
             // cancellation makes that estimate unreliable (the IFNEEDED criterion of the reference's KSP)
@@ -1017,7 +1017,7 @@ inline int Solver::solveLinearEqn(const double* rhs, double* sol, KspStats& st)
                 const double* d2 = K.ops.dots(K.V.p, n, k + 2, vk1, n);
                 std::vector<double> h2(d2, d2 + k + 1);
                 const double wn2b = d2[k + 1];
-                be.h2d(K.hdev.p, h2.data(), (size_t)(k + 1) * sizeof(double));
+                K.putCoeffs(be, h2.data(), k + 1);
                 be.launch(n, MultiAxpy{K.V.p, n, k + 1, K.hdev.p, vk1, 0});
                 double h2n = 0.0;
                 for (int j = 0; j <= k; j++)
@@ -1062,7 +1062,7 @@ inline int Solver::solveLinearEqn(const double* rhs, double* sol, KspStats& st)
             for (int j = i + 1; j < k; j++) s -= H[(size_t)i * m + j] * yv[j];
             yv[i] = s / H[(size_t)i * m + i];
         }
-        be.h2d(K.hdev.p, yv.data(), (size_t)k * sizeof(double));
+        K.putCoeffs(be, yv.data(), k);
         be.launch(n, MultiAxpy{K.V.p, n, k, K.hdev.p, K.w.p, 1});
         applyPC(K.w.p, K.z.p);
         be.launch(n, AxpyVec{K.z.p, 1.0, K.xdev.p});
@@ -1122,12 +1122,15 @@ inline int Solver::solveIdrs(const double* rhs, double* sol, KspStats& st)
         K.idrS = s;
         K.xdev.alloc(be, n);
         K.bdev.alloc(be, n);
-        K.hdev.alloc(be, std::max(gmresRestart, 32) + 2);
         K.ops.init(be, &comm, std::max(gmresRestart, 32) + 2);
-        K.vCap = 0; // the GMRES basis (if any) shares nothing with this workspace; hdev/ops were re-sized
+        K.vCap = 0; // the GMRES basis (if any) shares nothing with this workspace
         K.V.alloc(be, 1, false);
         K.idrShadowReady = false;
     }
+    // the coefficient buffer and the dot-product workspace are shared with GMRES, which may have re-sized them since this
+    // workspace was made (IDR(s), GMRES(m < s - 1), IDR(s) on one handle): both only grow
+    if (K.hdev.n < (size_t)s) K.hdev.alloc(be, s);
+    K.ops.init(be, &comm, s);
     double* P = K.idr.p;
     double* G = P + (size_t)s * n;
     double* U = G + (size_t)s * n;
@@ -1196,7 +1199,7 @@ inline int Solver::solveIdrs(const double* rhs, double* sol, KspStats& st)
                     for (int j = k; j < i; j++) a -= M[(size_t)i * s + j] * c[j];
                     c[i] = a / M[(size_t)i * s + i];
                 }
-                be.h2d(K.hdev.p, c.data() + k, (size_t)(s - k) * sizeof(double));
+                K.putCoeffs(be, c.data() + k, s - k);
                 be.d2d(v, r, (size_t)n * sizeof(double));
                 be.launch(n, MultiAxpy{G + (size_t)k * n, n, s - k, K.hdev.p, v, 0}); // v = r - sum c_i G_i
                 applyPC(v, z);
@@ -1224,7 +1227,7 @@ inline int Solver::solveIdrs(const double* rhs, double* sol, KspStats& st)
                     }
                     if (k > 0)
                     {
-                        be.h2d(K.hdev.p, al.data(), (size_t)k * sizeof(double));
+                        K.putCoeffs(be, al.data(), k);
                         be.launch(n, MultiAxpy{G, n, k, K.hdev.p, Gk, 0}); // Gk -= sum_i al_i G_i
                         be.launch(n, MultiAxpy{U, n, k, K.hdev.p, Uk, 0}); // Uk -= sum_i al_i U_i
                     }
