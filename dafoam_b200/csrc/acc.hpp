@@ -41,7 +41,7 @@ struct GAcc
     // ---- face data
     DAB_HD void Sf(int f, double* v) const { v[0] = m.Sx[f]; v[1] = m.Sy[f]; v[2] = m.Sz[f]; }
     DAB_HD void kv(int f, double* v) const { v[0] = m.kx[f]; v[1] = m.ky[f]; v[2] = m.kz[f]; }
-    DAB_HD void Cf(int f, double* v) const { v[0] = m.Cfx[f]; v[1] = m.Cfy[f]; v[2] = m.Cfz[f]; }
+    DAB_HD void faceOff(int f, double* dO, double* dN) const { faceOffsets(m, f, dO, dN); }
     DAB_HD double magSf(int f) const { return m.magSf[f]; }
     DAB_HD double w(int f) const { return m.w[f]; }
     DAB_HD double delta(int f) const { return m.delta[f]; }
@@ -50,7 +50,6 @@ struct GAcc
     // ---- cell data: mesh, state, input vector
     DAB_HD double V(int c) const { return m.V[c]; }
     DAB_HD double yWall(int c) const { return m.yWall[c]; }
-    DAB_HD double C(int c, int j) const { return (j == 0 ? m.Cx : (j == 1 ? m.Cy : m.Cz))[c]; }
     DAB_HD double U(int c, int j) const { return s.U[3 * c + j]; }
     DAB_HD double p(int c) const { return s.p[c]; }
     DAB_HD double nt(int c) const { return s.nt[c]; }

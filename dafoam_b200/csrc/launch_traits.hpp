@@ -15,7 +15,7 @@ namespace dab
 
 #if !defined(DAB_HOSTSIM)
 // RevB: at 2 CTAs per SM (up to 255 registers) a face's whole load block stays in registers; at 3 (168 registers) the kernel
-// spills and is a third slower on the H100, at 4 (128) more than twice as slow (DESIGN.md section 4)
+// spills and is 40 % slower on the H100, at 4 (128) more than twice as slow (DESIGN.md section 4)
 #ifndef DAB_REVB_MINBLOCKS
 #define DAB_REVB_MINBLOCKS 2
 #endif

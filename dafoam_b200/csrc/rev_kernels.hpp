@@ -297,8 +297,10 @@ DAB_HD void diagAdj(double Dn, double fl, double rAl, const double* mt, const do
 // A cell's ELL row lists its internal faces before its boundary faces (HostMesh::checkEllOrder), so the face loop is two passes
 // over the row: the internal pass gathers the neighbour's record with every face, the boundary pass reads only the face and the
 // cell itself.  The slots are visited in row order either way: the accumulation order is that of one loop.  Cell values that
-// are cheap to re-read (centre, volume, wall distance, grad nuTilda: L1 hits) or to recompute (trace of grad U, the SA
-// diffusivity, the diagonal scalars) are not held across the faces, so that the internal pass's load block stays in registers.
+// are cheap to re-read (volume, wall distance, grad nuTilda: L1 hits) or to recompute (trace of grad U, the SA diffusivity, the
+// diagonal scalars) are not held across the faces, so that the internal pass's load block stays in registers.  The face centre
+// enters only through its offsets from the two cells, which the mesh stores per face (MeshView::offOwn / offNei): six face loads
+// instead of the face centre and the two cell centres.
 template <int NF, int FEAT, class Acc>
 DAB_HD void revBCell(const Acc& A, const Params& q, int c, bool gradOnly)
 {
@@ -333,20 +335,18 @@ DAB_HD void revBCell(const Acc& A, const Params& q, int c, bool gradOnly)
         // ---- load block (see revACell): the face's geometry and flux and the neighbour's record, issued with no control flow in
         // between
         const double phi = A.phi(f), xphif = A.xphi(f);
-        double Sv[3], kv[3], Cfv[3];
+        double Sv[3], kv[3], dO[3], dN[3];
         A.Sf(f, Sv);
         A.kv(f, kv);
-        A.Cf(f, Cfv);
+        A.faceOff(f, dO, dN);
         const double mS = A.magSf(f), dl = A.delta(f), wf = A.w(f);
         const double Un[3] = {A.U(n, 0), A.U(n, 1), A.U(n, 2)};
         const double nutn = A.nut(n), Dnn = A.Dn(n), fln = A.flag(n), Vn = A.V(n);
         const double mtn[3] = {A.mt(n, 0), A.mt(n, 1), A.mt(n, 2)};
-        const double Cn[3] = {A.C(n, 0), A.C(n, 1), A.C(n, 2)};
         double gUn[9], gNn[3];
         for (int i = 0; i < 9; i++) gUn[i] = A.gU(n, i);
         const double ntn = q.turb ? A.nt(n) : 0.0, xntn = q.turb ? A.xnt(n) : 0.0;
         for (int i = 0; i < 3; i++) gNn[i] = q.turb ? A.gNt(n, i) : 0.0;
-        const double Cc[3] = {A.C(c, 0), A.C(c, 1), A.C(c, 2)};
         double gNc[3];
         for (int i = 0; i < 3; i++) gNc[i] = q.turb ? A.gNt(c, i) : 0.0;
         const double mf = fr.s * phi;
@@ -361,7 +361,9 @@ DAB_HD void revBCell(const Acc& A, const Params& q, int c, bool gradOnly)
         diagAdj(Dnn, fln, rAl, mtn, Un, D1n, son, D0n);
         const bool ownUp = phi > 0.0;
         const bool cUp = fr.s > 0 ? ownUp : !ownUp;
-        const double dC[3] = {Cfv[0] - Cc[0], Cfv[1] - Cc[1], Cfv[2] - Cc[2]};
+        // offsets of the face centre from this cell (dC) and from the neighbour (dX): Cf - C_c, Cf - C_n
+        const double dC[3] = {fr.s > 0 ? dO[0] : dN[0], fr.s > 0 ? dO[1] : dN[1], fr.s > 0 ? dO[2] : dN[2]};
+        const double dX[3] = {fr.s > 0 ? dN[0] : dO[0], fr.s > 0 ? dN[1] : dO[1], fr.s > 0 ? dN[2] : dO[2]};
         // ---- momentum rows c and n
         {
             const double wpc = schU == DIV_LINEAR ? wc : wupc;
@@ -395,7 +397,7 @@ DAB_HD void revBCell(const Acc& A, const Params& q, int c, bool gradOnly)
                     {
                         // per-element selects: a pointer into either gradient array would put both in local memory
                         double d[3];
-                        for (int i = 0; i < 3; i++) d[i] = cUp ? dC[i] : Cfv[i] - Cn[i];
+                        for (int i = 0; i < 3; i++) d[i] = cUp ? dC[i] : dX[i];
                         for (int j = 0; j < 3; j++)
                         {
                             const double gu0 = cUp ? gUc[j * 3 + 0] : gUn[j * 3 + 0], gu1 = cUp ? gUc[j * 3 + 1] : gUn[j * 3 + 1],
@@ -410,7 +412,7 @@ DAB_HD void revBCell(const Acc& A, const Params& q, int c, bool gradOnly)
                 double gu[9]; // per-element selects: a pointer into either array would put both in local memory
                 for (int i = 0; i < 9; i++) gu[i] = cUp ? gUc[i] : gUn[i];
                 double d[3];
-                for (int i = 0; i < 3; i++) d[i] = cUp ? dC[i] : Cfv[i] - Cn[i];
+                for (int i = 0; i < 3; i++) d[i] = cUp ? dC[i] : dX[i];
                 double corr[3], corrL[3], outb[3], corrb[3] = {0, 0, 0};
                 for (int j = 0; j < 3; j++)
                 {
@@ -478,7 +480,7 @@ DAB_HD void revBCell(const Acc& A, const Params& q, int c, bool gradOnly)
                 if (fr.s > 0)
                 {
                     double corr = 0.0;
-                    for (int i = 0; i < 3; i++) corr += (cUp ? dC[i] * gNc[i] : (Cfv[i] - Cn[i]) * gNn[i]);
+                    for (int i = 0; i < 3; i++) corr += (cUp ? dC[i] * gNc[i] : dX[i] * gNn[i]);
                     phib_acc += corr * lam;
                 }
             }

@@ -217,6 +217,7 @@ struct Solver
     DevBuf<int32_t> dOwn, dNei, dCellFaces, dCellNbr, dBPatch;
     DevBuf<double> dS[3], dMagSf, dW, dDelta, dK[3], dCf[3], dV, dY;
     DevBuf<double> dC; // cell centres, SoA in one buffer (x | y | z, nCtot each): one halo item when the geometry is rebuilt
+    DevBuf<double> dFaceOff; // MeshView::offOwn | offNei ([3][nIF] each), rebuilt with the centres (updateFaceOffsets)
     MeshView mv;
     // state (internal working copies with ghost slots) and external-layout mirror
     DevBuf<double> dWext, dU, dP, dNt, dPhi, dT;
@@ -1020,6 +1021,9 @@ struct Solver
         mv.Sx = dS[0].p; mv.Sy = dS[1].p; mv.Sz = dS[2].p; mv.magSf = dMagSf.p; mv.w = dW.p; mv.delta = dDelta.p;
         mv.kx = dK[0].p; mv.ky = dK[1].p; mv.kz = dK[2].p; mv.Cfx = dCf[0].p; mv.Cfy = dCf[1].p; mv.Cfz = dCf[2].p;
         mv.Cx = dC.p; mv.Cy = dC.p + hm.nCtot; mv.Cz = dC.p + 2 * (size_t)hm.nCtot; mv.V = dV.p; mv.yWall = dY.p;
+        dFaceOff.alloc(be, (size_t)6 * hm.nIF, false);
+        mv.offOwn = dFaceOff.p; mv.offNei = dFaceOff.p + (size_t)3 * hm.nIF;
+        updateFaceOffsets();
         mv.fvS = nullptr;
         mv.mrfCell = nullptr; mv.mrfType = nullptr; mv.mrfFlux = nullptr;
         if (mrf.on)
@@ -1200,14 +1204,15 @@ struct Solver
         const size_t nT = hm.nCtot;
         pl.cell(sv.U, 24); pl.cell(rv.nut, 8); pl.cell(mv.V, 8); pl.cell(av.Dn, 8); pl.cell(rv.flag, 8);
         for (int i = 0; i < 9; i++) pl.cell(rv.gU + i * nT, 8);
-        for (int j = 0; j < 3; j++) { pl.cell(av.mt + j * nT, 8); pl.cell((j == 0 ? mv.Cx : (j == 1 ? mv.Cy : mv.Cz)), 8); }
+        for (int j = 0; j < 3; j++) pl.cell(av.mt + j * nT, 8);
         if (par.turb)
         {
             pl.cell(sv.nt, 8); pl.cell(pv.nt, 8); pl.cell(mv.yWall, 8);
             for (int j = 0; j < 3; j++) pl.cell(rv.gNt + j * nT, 8);
         }
         pl.face(sv.phi, 8); pl.face(mv.Sx, 8); pl.face(mv.Sy, 8); pl.face(mv.Sz, 8); pl.face(mv.magSf, 8); pl.face(mv.delta, 8); pl.face(mv.w, 8);
-        pl.face(mv.kx, 8); pl.face(mv.ky, 8); pl.face(mv.kz, 8); pl.face(mv.Cfx, 8); pl.face(mv.Cfy, 8); pl.face(mv.Cfz, 8); pl.face(pv.phi, 8);
+        // not the face-centre offsets: they have internal faces only, and a chunk's face ranges include boundary faces
+        pl.face(mv.kx, 8); pl.face(mv.ky, 8); pl.face(mv.kz, 8); pl.face(pv.phi, 8);
         return pl;
     }
     PfPlan pfRevC() const
@@ -2392,6 +2397,7 @@ struct Solver
     VolCoord volc;
     void uploadGeometry();
     void deviceGeometry();
+    void updateFaceOffsets() { be.launch(hm.nIF, FaceOffsetK{mv, dFaceOff.p, dFaceOff.p + (size_t)3 * hm.nIF}); }
     void downloadGeometry();
     void updateMesh(const double* pts);
     void volCoordSetup();

@@ -21,6 +21,7 @@ inline void Solver::uploadGeometry()
     put(dW.p, hm.w);
     put(dDelta.p, hm.delta);
     put(dV.p, hm.V);
+    updateFaceOffsets();
     updateMrfFlux();
     recorded = false;
     kry.pcValid = false;
@@ -76,6 +77,7 @@ inline void Solver::deviceGeometry()
         halo.exchangeCells({centres, {dV.p, 1, 1, (int)nT}});
     }
     be.launch(hm.nF, GeomDerivedK{gv});
+    updateFaceOffsets();
 }
 
 // new point coordinates (the wall distance stays frozen: meshWaveFrozen).  Every rank passes the same full point list.

@@ -21,7 +21,7 @@ namespace dab
 // capacities compiled into the tile kernels (doubles per array are EXT*, shared memory is static per program)
 constexpr int TILE_TMAX = 192; // cells per tile (= threads per CTA: 6 warps)
 constexpr int TILE_EXT1 = 256; // tile + ring 1
-constexpr int TILE_EXT2 = 320; // tile + rings 1, 2   (ProdTileBC: 110.8 KB of shared memory -> 2 CTAs per SM)
+constexpr int TILE_EXT2 = 320; // tile + rings 1, 2   (ProdTileBC: 101 888 B of shared memory -> 2 CTAs per SM)
 
 // shared base of the tile accessors: topology of the current tile + face data from global memory
 struct TAccBase
@@ -48,7 +48,7 @@ struct TAccBase
     DAB_HD int patch(int f) const { return m.bPatch[f - m.nIF]; }
     DAB_HD void Sf(int f, double* v) const { v[0] = m.Sx[f]; v[1] = m.Sy[f]; v[2] = m.Sz[f]; }
     DAB_HD void kv(int f, double* v) const { v[0] = m.kx[f]; v[1] = m.ky[f]; v[2] = m.kz[f]; }
-    DAB_HD void Cf(int f, double* v) const { v[0] = m.Cfx[f]; v[1] = m.Cfy[f]; v[2] = m.Cfz[f]; }
+    DAB_HD void faceOff(int f, double* dO, double* dN) const { faceOffsets(m, f, dO, dN); }
     DAB_HD double magSf(int f) const { return m.magSf[f]; }
     DAB_HD double w(int f) const { return m.w[f]; }
     DAB_HD double delta(int f) const { return m.delta[f]; }
@@ -139,7 +139,7 @@ struct TAccBC : TAccBase
     enum
     {
         O_U = 0, O_NUT = 3 * E2, O_MT = 4 * E2, O_DN = 7 * E2, O_FLAG = 8 * E2, O_GU = 9 * E2, O_NT = 18 * E2, O_XNT = 19 * E2,
-        O_V = 20 * E2, O_GNT = 21 * E2, O_C = 24 * E2, END2 = 27 * E2,
+        O_V = 20 * E2, O_GNT = 21 * E2, END2 = 24 * E2,
         // tile + ring 1 (RevC reads the gradient adjoints of the neighbours)
         O_GPB = END2, O_GUB = END2 + 3 * E1, O_GNTB = END2 + 12 * E1, O_YW = END2 + 15 * E1, END1 = END2 + 16 * E1,
         // tile only (RevB -> RevC of the same cell)
@@ -158,7 +158,6 @@ struct TAccBC : TAccBase
     DAB_HD double xnt(int c) const { return sm[O_XNT + c]; }
     DAB_HD double V(int c) const { return sm[O_V + c]; }
     DAB_HD double gNt(int c, int i) const { return sm[O_GNT + i * E2 + c]; }
-    DAB_HD double C(int c, int j) const { return sm[O_C + j * E2 + c]; }
     DAB_HD double yWall(int c) const { return sm[O_YW + c]; }
     DAB_HD double gPb(int c, int i) const { return sm[O_GPB + i * E1 + c]; }
     DAB_HD double gUb(int c, int i) const { return sm[O_GUB + i * E1 + c]; }
@@ -218,9 +217,6 @@ struct ProdTileBC
                 sm[TAccBC::O_XNT + l] = q.turb ? x.nt[g] : 0.0;
                 sm[TAccBC::O_V + l] = m.V[g];
                 for (int i = 0; i < 3; i++) sm[TAccBC::O_GNT + i * E2 + l] = q.turb ? r.gNt[(size_t)i * nTg + g] : 0.0;
-                sm[TAccBC::O_C + l] = m.Cx[g];
-                sm[TAccBC::O_C + E2 + l] = m.Cy[g];
-                sm[TAccBC::O_C + 2 * E2 + l] = m.Cz[g];
                 if (l < n1)
                 {
                     for (int i = 0; i < 3; i++) sm[TAccBC::O_GPB + i * E1 + l] = a.gPb[(size_t)i * nTg + g];

@@ -45,6 +45,8 @@ struct MeshView
     const int32_t* bPatch;    // [nBF]
     const double *Sx, *Sy, *Sz, *magSf, *w, *delta, *kx, *ky, *kz, *Cfx, *Cfy, *Cfz; // [nF]
     const double *Cx, *Cy, *Cz, *V, *yWall;                                          // [nCtot]
+    // face-centre offsets of the internal faces, SoA [3][nIF]: offOwn = Cf - C[own], offNei = Cf - C[nei] (FaceOffsetK)
+    const double *offOwn, *offNei;
     const double* fvS; // [3][nC] momentum source per unit volume (fvSource: actuator disks) or null
     // MRF zone (reference src/adjoint/DAMisc/MRFDF/MRFZoneDF.C) or null pointers: cell mask, boundary-face type
     // (MRFZoneDF::setMRFFaces: 1 included = rotating wall, 2 excluded), (Omega x (Cf - origin)) . Sf of the zone faces
@@ -98,6 +100,37 @@ struct MrfFluxK
         out[f] = v;
     }
 };
+
+// offOwn / offNei of the internal faces from the face and cell centres (ghost and periodic-image slots included).  They depend on
+// the geometry only, so the transpose product reads them instead of gathering the two cell centres on every face; the solver
+// rebuilds them wherever it writes the centres (Solver::updateFaceOffsets)
+struct FaceOffsetK
+{
+    MeshView m;
+    double *offOwn, *offNei;
+    DAB_HD void operator()(int f) const
+    {
+        const size_t nIF = m.nIF;
+        const int o = m.own[f], n = m.nei[f];
+        offOwn[f] = m.Cfx[f] - m.Cx[o]; offOwn[nIF + f] = m.Cfy[f] - m.Cy[o]; offOwn[2 * nIF + f] = m.Cfz[f] - m.Cz[o];
+        offNei[f] = m.Cfx[f] - m.Cx[n]; offNei[nIF + f] = m.Cfy[f] - m.Cy[n]; offNei[2 * nIF + f] = m.Cfz[f] - m.Cz[n];
+    }
+};
+
+// the offsets of internal face f as the transpose product reads them.  DAB_FACE_OFFSETS_FROM_CENTRES (a test-only host build,
+// tests/test_face_offsets.py) takes the same differences from the centres on every call: the product must not change by a bit
+DAB_HD void faceOffsets(const MeshView& m, int f, double* dO, double* dN)
+{
+#if defined(DAB_FACE_OFFSETS_FROM_CENTRES)
+    const int o = m.own[f], n = m.nei[f];
+    dO[0] = m.Cfx[f] - m.Cx[o]; dO[1] = m.Cfy[f] - m.Cy[o]; dO[2] = m.Cfz[f] - m.Cz[o];
+    dN[0] = m.Cfx[f] - m.Cx[n]; dN[1] = m.Cfy[f] - m.Cy[n]; dN[2] = m.Cfz[f] - m.Cz[n];
+#else
+    const size_t nIF = m.nIF;
+    dO[0] = m.offOwn[f]; dO[1] = m.offOwn[nIF + f]; dO[2] = m.offOwn[2 * nIF + f];
+    dN[0] = m.offNei[f]; dN[1] = m.offNei[nIF + f]; dN[2] = m.offNei[2 * nIF + f];
+#endif
+}
 
 // DAFvSourceActuatorDisk, source = cylinderAnnulusSmooth (reference src/adjoint/DAFvSource/DAFvSourceActuatorDisk.C:205-407):
 // the 13 actuatorDiskPars (center, direction, innerRadius, outerRadius, scale, POD, expM, expN, targetThrust) + eps, rotDir
