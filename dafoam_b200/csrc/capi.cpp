@@ -499,6 +499,15 @@ int dab_get_pc_aggregates(dab_solver* s, int32_t* agg_of)
     DAB_CATCH
 }
 
+int dab_get_face_loop_width(dab_solver* s, int* nf)
+{
+    DAB_TRY
+    need(s, "solver");
+    need(nf, "nf");
+    *nf = s->s.hex6 ? 6 : 0;
+    DAB_CATCH
+}
+
 int dab_calc_pc_mat_fvmatrix(dab_solver* s, int turb_only, int64_t* nnz, int32_t* rows, int32_t* cols, double* vals)
 {
     DAB_TRY

@@ -601,6 +601,12 @@ class pyDASolvers:
         self._raise(self._L.dab_get_pc_aggregates(self._h, agg.ctypes.data_as(C.POINTER(C.c_int32))))
         return agg
 
+    def getFaceLoopWidth(self):
+        """Test hook: 6 when the cell-per-thread kernels run the unrolled six-face loops, 0 for the rolled loops."""
+        nf = C.c_int()
+        self._raise(self._L.dab_get_face_loop_width(self._h, C.byref(nf)))
+        return nf.value
+
     def initializedRdWTMatrixFree(self):
         return None
 

@@ -201,6 +201,11 @@ int dab_get_pc_factors(dab_solver* s, int64_t* n_rows, int64_t* nnz, int64_t* ro
  * space (adjEqnOption.coarseAggregates > 0); an error without a coarse space. */
 int dab_get_pc_aggregates(dab_solver* s, int32_t* agg_of);
 
+/* Test hook (no counterpart in the reference): the face-loop width of the cell-per-thread kernels this solver launches -- 6 when
+ * every owned cell has exactly six faces (the unrolled NF=6 instantiations), 0 otherwise or with DAB_NOHEX6=1 at creation (the
+ * rolled NF=0 loops). */
+int dab_get_face_loop_width(dab_solver* s, int* nf);
+
 /* calcPCMatWithFvMatrix(PCMat, turbOnly) (reference pyDASolvers.pyx:99-114 list, DASolver.C:2888-2988): the turbulence block of
  * the preconditioner taken from the relaxed nuTilda fvMatrix (diag / lower / upper, `div(pc)` convection, DASpalartAllmaras.C:
  * 490-529), scaled and transposed like the reference, as COO triplets (row, column, value) in the local state numbering -- what the
