@@ -353,11 +353,18 @@ int dab_calc_jac_t_vec_product(dab_solver* s, const char* input_name, const char
             for (size_t i = 0; i < S.hm.points.size() && same; i++) same = (input[i] == S.hm.points[i]);
             if (!same) S.updateMesh(input);
         }
-        if (ot == "residual") S.volCoordProduct(seed, nullptr, 1.0, product);
+        if (ot == "residual") S.volCoordProduct(seed, {}, 1.0, product);
         else if (ot == "function")
         {
             need(output_name, "output_name");
-            S.volCoordProduct(nullptr, &S.findFunction(output_name), seed[0], product);
+            const FunctionDef& f = S.findFunction(output_name);
+            S.ensureRecorded();
+            S.volCoordProduct(nullptr, S.derivativeSpecs(f), seed[0], product); // at the unperturbed geometry
+        }
+        else if (ot == "forceCouplingOutput")
+        {
+            need(output_name, "output_name");
+            S.forceCouplingdXv(output_name, seed, product);
         }
         else throw Error("calcJacTVecProduct: outputType " + ot + " is not supported");
         return 0;
@@ -371,7 +378,12 @@ int dab_calc_jac_t_vec_product(dab_solver* s, const char* input_name, const char
         need(output_name, "output_name");
         S.dFdW(output_name, seed[0], product);
     }
-    else throw Error("calcJacTVecProduct: outputType " + ot + " is not supported (residual, function)");
+    else if (ot == "forceCouplingOutput")
+    {
+        need(output_name, "output_name");
+        S.forceCouplingdW(output_name, seed, product);
+    }
+    else throw Error("calcJacTVecProduct: outputType " + ot + " is not supported (residual, function, forceCouplingOutput)");
     DAB_CATCH
 }
 
@@ -686,11 +698,39 @@ int dab_get_output_size(dab_solver* s, const char* name, const char* type, int64
     DAB_TRY
     need(s, "solver");
     need(type, "type");
-    (void)name;
     const std::string t(type);
     if (t == "residual") *out = s->s.nDof();
     else if (t == "function") *out = 1;
+    else if (t == "forceCouplingOutput")
+    {
+        need(name, "name");
+        *out = s->s.couplingSize(name);
+    }
     else throw Error("getOutputSize: unsupported output type " + t);
+    DAB_CATCH
+}
+
+int dab_calc_output(dab_solver* s, const char* name, const char* type, double* out)
+{
+    DAB_TRY
+    need(s, "solver");
+    need(name, "name");
+    need(type, "type");
+    need(out, "out");
+    const std::string t(type);
+    if (t != "forceCouplingOutput") throw Error("calcOutput: output type " + t + " is not supported (forceCouplingOutput)");
+    s->s.calcForceCoupling(name, out);
+    DAB_CATCH
+}
+
+int dab_get_output_points(dab_solver* s, const char* name, int64_t* labels)
+{
+    DAB_TRY
+    need(s, "solver");
+    need(name, "name");
+    need(labels, "labels");
+    const std::vector<int64_t>& n = s->s.findForceCoupling(name).nodes;
+    std::copy(n.begin(), n.end(), labels);
     DAB_CATCH
 }
 

@@ -803,8 +803,9 @@ struct cRevC
 };
 
 // ---- force / moment function (DAFunctionForce.C:79-153 with the compressible devRhoReff = -rho*nuEff*dev(twoSymm(grad U)))
+// fv (optional, modes 0, 1): the face's force vector Sf (p_b - pRef) + Sf & devRhoReff_b
 DAB_HD double cForceFace(const MeshView& m, const Params& q, const StateView& s, const RecordView& r, const ForceSpec& fs, int f, int c,
-                         double seed, double* Ub, double* pb, double* Tb, double* ntb, double* nutPb, double* gUb)
+                         double seed, double* Ub, double* pb, double* Tb, double* ntb, double* nutPb, double* gUb, double* fv = nullptr)
 {
     const int nT = m.nCtot;
     const double mS = m.magSf[f];
@@ -870,7 +871,9 @@ DAB_HD double cForceFace(const MeshView& m, const Params& q, const StateView& s,
     }
     const double trb = Gbd[0] + Gbd[4] + Gbd[8];
     double ed[3] = {fs.dir[0], fs.dir[1], fs.dir[2]};
-    if (fs.mode == 1)
+    if (fs.faceDir)
+        for (int j = 0; j < 3; j++) ed[j] = fs.faceDir[3 * (f - m.nIF) + j];
+    else if (fs.mode == 1)
     {
         const double rv[3] = {m.Cfx[f] - fs.center[0], m.Cfy[f] - fs.center[1], m.Cfz[f] - fs.center[2]};
         ed[0] = fs.dir[1] * rv[2] - fs.dir[2] * rv[1];
@@ -883,7 +886,9 @@ DAB_HD double cForceFace(const MeshView& m, const Params& q, const StateView& s,
         double t = 0.0;
         for (int i = 0; i < 3; i++) t += Sv[i] * (Gbd[j * 3 + i] + Gbd[i * 3 + j]);
         sj[j] = t - (2.0 / 3.0) * trb * Sv[j];
-        F += (Sv[j] * bp.p - bp.muE * sj[j]) * ed[j];
+        const double fj = Sv[j] * (bp.p - fs.pRef) - bp.muE * sj[j];
+        if (fv) fv[j] = fj;
+        F += fj * ed[j];
     }
     F *= fs.scale;
     if (gUb)

@@ -761,11 +761,14 @@ struct ForceSpec
     double shift = 0.0;  // modes 2, 4: subtracted from the face value before the area weighting; with shift = the average itself
                          // the geometric derivative of the area average needs no derivative of areaSum
     int accumulate = 0;  // ForceFwd: leave the faces outside the mask untouched (a second face group)
+    double pRef = 0.0;   // modes 0, 1: reference pressure subtracted from the wall pressure (forceCouplingOutput)
+    const double* faceDir = nullptr; // modes 0, 1: per-face direction [3*nBF] (by boundary face) in place of dir; null: dir
 };
 
 // boundary-face force contribution and (optionally) its adjoint w.r.t. the cell's variables
+// fv (optional, modes 0, 1): the face's force vector Sf (p_b - pRef) + Sf & devRhoReff_b
 DAB_HD double forceFace(const MeshView& m, const Params& q, const StateView& s, const RecordView& r, const ForceSpec& fs, int f, int c,
-                        double seed, double* Ub, double* pb, double* ntb_, double* nutPb, double* gUb)
+                        double seed, double* Ub, double* pb, double* ntb_, double* nutPb, double* gUb, double* fv = nullptr)
 {
     const int nT = m.nCtot;
     const int b = f - m.nIF, pa = m.bPatch[b];
@@ -815,7 +818,9 @@ DAB_HD double forceFace(const MeshView& m, const Params& q, const StateView& s, 
     const double trb = Gbd[0] + Gbd[4] + Gbd[8];
     // effective direction of this face: dir for a force, axis x r for a moment ((r x F).a = F.(a x r))
     double ed[3] = {fs.dir[0], fs.dir[1], fs.dir[2]};
-    if (fs.mode == 1)
+    if (fs.faceDir)
+        for (int j = 0; j < 3; j++) ed[j] = fs.faceDir[3 * b + j];
+    else if (fs.mode == 1)
     {
         const double rv[3] = {m.Cfx[f] - fs.center[0], m.Cfy[f] - fs.center[1], m.Cfz[f] - fs.center[2]};
         ed[0] = fs.dir[1] * rv[2] - fs.dir[2] * rv[1];
@@ -829,7 +834,9 @@ DAB_HD double forceFace(const MeshView& m, const Params& q, const StateView& s, 
         double t = 0.0;
         for (int i = 0; i < 3; i++) t += Sv[i] * (Gbd[j * 3 + i] + Gbd[i * 3 + j]);
         sj[j] = t - (2.0 / 3.0) * trb * Sv[j];
-        F += (Sv[j] * pv - nuEB * sj[j]) * ed[j];
+        const double fj = Sv[j] * (pv - fs.pRef) - nuEB * sj[j];
+        if (fv) fv[j] = fj;
+        F += fj * ed[j];
     }
     F *= fs.scale;
     if (gUb)

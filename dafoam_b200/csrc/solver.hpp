@@ -16,6 +16,7 @@
 #include "tile_kernels.hpp"
 #include "comp_kernels.hpp"
 #include "comp_rev_kernels.hpp"
+#include "coupling_kernels.hpp"
 #include "krylov.hpp"
 #include "primal_kernels.hpp"
 #include "geom_kernels.hpp"
@@ -139,6 +140,19 @@ struct FunctionDef
     double scale = 1.0;
 };
 
+// DAOutputForceCoupling (reference src/adjoint/DAOutput/DAOutputForceCoupling.C): an outputInfo entry of type forceCouplingOutput.
+// The tables depend on the topology only (couplingTables), so they outlive updateOFMesh.
+struct OutputDef
+{
+    std::string name, type;      // other types are kept by name and rejected when used
+    std::vector<int> patches;    // sorted by name: the output follows that order (DAOutputForceCoupling.C:41)
+    double pRef = 0.0;
+    std::vector<int64_t> nodes;  // point label of every output node (global on a partitioned mesh), in output order
+    CouplingView cv{};
+    DevBuf<int32_t> dFace, dFsOff, dFsLab, dNfOff, dNfLab;
+    DevBuf<double> dFaceF, dSeed, dFaceDir;
+};
+
 // work data of the volCoord input (solver_volcoord.hpp)
 struct VolCoord
 {
@@ -190,6 +204,7 @@ struct Solver
     int coarseAggregates = 0; // > 0: two-level preconditioner with that many pressure aggregates (global)
     int pcConLevel = 2; // cell-to-cell connectivity level of dRdWTPC (maxResConLv4JacPCMat role)
     std::vector<FunctionDef> functions;
+    std::map<std::string, OutputDef> outputs; // outputInfo
     std::vector<PatchVelocityDef> patchVelocities;
     std::vector<PatchVarDef> patchVars;
     // fvSource (actuator disks) and the fvSourcePar inputs that address its parameters
@@ -988,8 +1003,77 @@ struct Solver
                 patchVelocities.push_back(d);
             }
         }
+        if (const JVal* oi = o.get("outputInfo"))
+        {
+            outputs.clear();
+            for (const auto& kv : oi->obj)
+            {
+                OutputDef& d = outputs[kv.first];
+                d.name = kv.first;
+                d.type = kv.second.strOr("type", "");
+                if (d.type != "forceCouplingOutput") continue;
+                if (const JVal* pl = kv.second.get("patches"))
+                    for (const auto& pn : pl->arr)
+                    {
+                        int found = -1;
+                        for (size_t p = 0; p < hm.patches.size(); p++)
+                            if (hm.patches[p].name == pn.str) found = (int)p;
+                        if (found < 0) throw Error("outputInfo " + d.name + ": unknown patch " + pn.str);
+                        if (std::find(d.patches.begin(), d.patches.end(), found) == d.patches.end()) d.patches.push_back(found);
+                    }
+                if (d.patches.empty()) throw Error("outputInfo " + d.name + ": patches is required");
+                const JVal* pr = kv.second.get("pRef");
+                if (!pr || pr->kind != JVal::Num) throw Error("outputInfo " + d.name + ": pRef is required");
+                d.pRef = pr->num;
+                std::sort(d.patches.begin(), d.patches.end(), [&](int a, int b) { return hm.patches[a].name < hm.patches[b].name; });
+                couplingTables(d);
+            }
+        }
         (void)first;
         recorded = false;
+    }
+
+    // the output slots of a forceCouplingOutput: per patch (sorted by name) its unique point labels in ascending order
+    // (DAOutputForceCoupling.C:194-201); then face -> slots and slot -> faces, both in increasing face order
+    void couplingTables(OutputDef& d)
+    {
+        std::vector<int32_t> face, fsOff{0}, fsLab;
+        d.nodes.clear();
+        for (int p : d.patches)
+        {
+            const PatchDef& pd = hm.patches[p];
+            const int base = (int)d.nodes.size();
+            std::vector<int32_t> lab;
+            for (int i = 0; i < pd.size; i++)
+                lab.insert(lab.end(), hm.fLab.begin() + hm.fOff[pd.start + i], hm.fLab.begin() + hm.fOff[pd.start + i + 1]);
+            std::sort(lab.begin(), lab.end());
+            lab.erase(std::unique(lab.begin(), lab.end()), lab.end());
+            d.nodes.insert(d.nodes.end(), lab.begin(), lab.end());
+            for (int i = 0; i < pd.size; i++)
+            {
+                const int f = pd.start + i;
+                face.push_back(f - hm.nIF);
+                for (int q = hm.fOff[f]; q < hm.fOff[f + 1]; q++)
+                    fsLab.push_back(base + (int32_t)(std::lower_bound(lab.begin(), lab.end(), hm.fLab[q]) - lab.begin()));
+                fsOff.push_back((int32_t)fsLab.size());
+            }
+        }
+        const int nN = (int)d.nodes.size(), nFc = (int)face.size();
+        std::vector<int32_t> nfOff(nN + 1, 0), nfLab(fsLab.size());
+        for (int32_t sl : fsLab) nfOff[sl + 1]++;
+        for (int n = 0; n < nN; n++) nfOff[n + 1] += nfOff[n];
+        std::vector<int32_t> pos(nfOff.begin(), nfOff.end() - 1);
+        for (int i = 0; i < nFc; i++)
+            for (int q = fsOff[i]; q < fsOff[i + 1]; q++) nfLab[pos[fsLab[q]]++] = i;
+        d.dFace.upload(be, face);
+        d.dFsOff.upload(be, fsOff);
+        d.dFsLab.upload(be, fsLab);
+        d.dNfOff.upload(be, nfOff);
+        d.dNfLab.upload(be, nfLab);
+        d.dFaceF.alloc(be, (size_t)3 * nFc);
+        d.dSeed.alloc(be, (size_t)3 * nN);
+        d.dFaceDir.alloc(be, (size_t)3 * hm.nBF);
+        d.cv = CouplingView{nFc, nN, d.dFace.p, d.dFsOff.p, d.dFsLab.p, d.dNfOff.p, d.dNfLab.p};
     }
 
     void upload()
@@ -2166,11 +2250,18 @@ struct Solver
     {
         const FunctionDef& f = findFunction(name);
         ensureRecorded();
+        std::vector<ForceSpec> specs;
+        if (par.comp && f.type == "totalPressureRatio") specs = derivativeSpecs(f);
+        else specs.push_back(forceSpec(f));
+        forceRev(specs, seed, out);
+    }
+
+    // the state reverse of the boundary-face groups `specs` (their sweeps add): the reverse work arrays seeded by ForceRevA /
+    // cForceRevA, then RevC / cRevC with no face-flux dependence
+    void forceRev(const std::vector<ForceSpec>& specs, double seed, double* out)
+    {
         if (par.comp)
         {
-            std::vector<ForceSpec> specs;
-            if (f.type == "totalPressureRatio") specs = derivativeSpecs(f);
-            else specs.push_back(forceSpec(f));
             std::vector<double> part;
             for (size_t g = 0; g < specs.size(); g++)
             {
@@ -2196,7 +2287,7 @@ struct Solver
         be.zero(av.gUb, (size_t)9 * hm.nCtot * sizeof(double));
         be.zero(av.gPb, (size_t)3 * hm.nCtot * sizeof(double));
         be.zero(av.gNtb, (size_t)3 * hm.nCtot * sizeof(double));
-        DAB_LAUNCH_NF(hm.nC, ForceRevA, mv, par, sv, rv, av, forceSpec(f), seed);
+        DAB_LAUNCH_NF(hm.nC, ForceRevA, mv, par, sv, rv, av, specs[0], seed);
         if (ghosted())
         {
             std::vector<HaloItem> it{{av.gUb, 9, 1, hm.nCtot}};
@@ -2204,6 +2295,68 @@ struct Solver
         }
         DAB_LAUNCH_NF(hm.nC, RevC, mv, par, sv, rv, av, dY2.p, 1);
         be.d2h(out, dY2.p, (size_t)nDof() * sizeof(double));
+    }
+
+    // ---- forceCouplingOutput (DAOutputForceCoupling) -------------------------------------------------
+    OutputDef& findForceCoupling(const std::string& name)
+    {
+        auto it = outputs.find(name);
+        if (it == outputs.end()) throw Error("output " + name + " is not defined in outputInfo");
+        if (it->second.type != "forceCouplingOutput")
+            throw Error("output " + name + ": type " + it->second.type + " is not supported (forceCouplingOutput)");
+        return it->second;
+    }
+    int64_t couplingSize(const std::string& name) { return (int64_t)3 * findForceCoupling(name).cv.nNodes; }
+
+    // the listed faces as one force group; faceDir: the per-face directions of a seed (couplingFaceSeed), null for the forward
+    ForceSpec couplingSpec(const OutputDef& d, const double* faceDir) const
+    {
+        ForceSpec fs{};
+        fs.mask = 0;
+        for (int p : d.patches) fs.mask |= (1u << p);
+        fs.scale = 1.0;
+        fs.mode = 0;
+        fs.areaSum = 1.0;
+        fs.gamma = 1.4;
+        fs.pRef = d.pRef;
+        fs.faceDir = faceDir;
+        return fs;
+    }
+
+    // out[3 * nNodes]: the nodal forces, x y z per node
+    void calcForceCoupling(const std::string& name, double* out)
+    {
+        OutputDef& d = findForceCoupling(name);
+        ensureRecorded();
+        const ForceSpec fs = couplingSpec(d, nullptr);
+        if (par.comp) be.launch(d.cv.nFaces, CouplingFaceFwd<true>{mv, par, sv, rv, fs, d.cv, d.dFaceF.p});
+        else be.launch(d.cv.nFaces, CouplingFaceFwd<false>{mv, par, sv, rv, fs, d.cv, d.dFaceF.p});
+        be.launch(d.cv.nNodes, CouplingNodeSum{d.cv, d.dFaceF.p, d.dSeed.p});
+        be.d2h(out, d.dSeed.p, (size_t)3 * d.cv.nNodes * sizeof(double));
+    }
+
+    // seed [3 * nNodes] -> the per-face directions d_f of s . f = sum_f d_f . F_f (1 / nPoints_f is topology)
+    ForceSpec couplingFaceSeed(OutputDef& d, const double* seed)
+    {
+        be.h2d(d.dSeed.p, seed, (size_t)3 * d.cv.nNodes * sizeof(double));
+        be.launch(d.cv.nFaces, CouplingFaceSeed{d.cv, d.dSeed.p, d.dFaceDir.p});
+        return couplingSpec(d, d.dFaceDir.p);
+    }
+
+    // [d(s . f)/dW]^T, scaled by normalizeStates; pRef drops out
+    void forceCouplingdW(const std::string& name, const double* seed, double* out)
+    {
+        OutputDef& d = findForceCoupling(name);
+        ensureRecorded();
+        forceRev({couplingFaceSeed(d, seed)}, 1.0, out);
+    }
+
+    // d(s . f)/dx_v: the scalar boundary function sum_f d_f . F_f(x) through the coloured central differences
+    void forceCouplingdXv(const std::string& name, const double* seed, double* out)
+    {
+        OutputDef& d = findForceCoupling(name);
+        ensureRecorded();
+        volCoordProduct(nullptr, {couplingFaceSeed(d, seed)}, 1.0, out);
     }
 
     // ---- OpenFOAM field files (runTime.write() / DASolver::writeAdjointFields, DASolver.C:4055-4160) ---------------
@@ -2401,7 +2554,8 @@ struct Solver
     void downloadGeometry();
     void updateMesh(const double* pts);
     void volCoordSetup();
-    void volCoordProduct(const double* psi, const FunctionDef* function, double seed, double* out);
+    // fsv empty: [dR/dx_v]^T psi; else seed * d(sum of the face groups fsv)/dx_v, fsv taken at the unperturbed geometry
+    void volCoordProduct(const double* psi, const std::vector<ForceSpec>& fsv, double seed, double* out);
 
     // ---- primal (SIMPLE) ----------------------------------------------------------------------------
     Primal primal;

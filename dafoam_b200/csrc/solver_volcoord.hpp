@@ -263,8 +263,8 @@ inline void Solver::volCoordSetup()
         fprintf(stderr, "[dab200] volCoord: %d colours x %d slots, %d residual evaluations per product\n", Vc.nColours, Vc.maxSlots, Vc.nEval);
 }
 
-// out[3*nP] = [dR/dx_v]^T psi (function == nullptr) or seed * dF/dx_v
-inline void Solver::volCoordProduct(const double* psi, const FunctionDef* function, double seed, double* out)
+// out[3*nP] = [dR/dx_v]^T psi (fsv empty) or seed * dF/dx_v of the face groups fsv
+inline void Solver::volCoordProduct(const double* psi, const std::vector<ForceSpec>& fsv, double seed, double* out)
 {
     volCoordSetup();
     VolCoord& Vc = volc;
@@ -278,12 +278,7 @@ inline void Solver::volCoordProduct(const double* psi, const FunctionDef* functi
     be.d2d(Vc.dPts.p, Vc.dPts0.p, (size_t)3 * nP * sizeof(double));
     be.zero(Vc.dOut.p, (size_t)3 * nP * sizeof(double));
     const int ns = nCellStates(), offPhi = ns * nC;
-    std::vector<ForceSpec> fsv;
-    if (function)
-    {
-        ensureRecorded();
-        fsv = derivativeSpecs(*function); // at the unperturbed geometry
-    }
+    const bool function = !fsv.empty();
     auto evaluate = [&](double* Rdev, double* Fdev) {
         geometry();
         if (function)

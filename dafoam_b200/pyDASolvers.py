@@ -276,7 +276,7 @@ class pyDASolvers:
         return 1 if inputType in ("stateVar", "volCoord") else 0
 
     def getOutputDistributed(self, outputName, outputType):
-        return 1 if outputType == "residual" else 0
+        return 1 if outputType in ("residual", "forceCouplingOutput") else 0
 
     def calcJacTVecProduct(self, inputName, inputType, inputs, outputName, outputType, seeds, product):
         inputSize = self.getInputSize(inputName, inputType)
@@ -294,14 +294,25 @@ class pyDASolvers:
 
     def calcOutput(self, outputName, outputType, output):
         """output[:] = the value of one output object (reference pyDASolvers.pyx calcOutput -> DAOutput::run;
-        DAOutputFunction.C, DAOutputResidual.C).  The coupling outputs (force/thermal) are outside this path."""
+        DAOutputFunction.C, DAOutputResidual.C, DAOutputForceCoupling.C).  forceCouplingOutput: the nodal wall forces
+        (x, y, z per node) of this rank's faces on the output's patches, in the order of getForceCouplingPoints."""
         _check_array(output, self.getOutputSize(outputName, outputType), "output")
         if outputType == "function":
             output[0] = self.calcFunction(outputName)
         elif outputType == "residual":
             self.getResiduals(output)
+        elif outputType == "forceCouplingOutput":
+            self._raise(self._L.dab_calc_output(self._h, outputName.encode(), outputType.encode(), _dp(output)))
         else:
-            raise DAB200Error("calcOutput: output type %s is not supported (function, residual)" % outputType)
+            raise DAB200Error("calcOutput: output type %s is not supported (function, residual, forceCouplingOutput)" % outputType)
+
+    def getForceCouplingPoints(self, outputName):
+        """The global point index of every node of a forceCouplingOutput, in output order: patches sorted by name, each patch's
+        points in ascending order (a point shared by two patches appears once per patch; on several ranks, a point on a partition
+        seam appears on every rank with faces around it)."""
+        out = np.zeros(self.getOutputSize(outputName, "forceCouplingOutput") // 3, dtype=np.int64)
+        self._raise(self._L.dab_get_output_points(self._h, outputName.encode(), out.ctypes.data_as(C.POINTER(C.c_int64))))
+        return out
 
     def calcPrimalResidualStatistics(self, mode):
         """Norm2 / mean / max of every residual block of this rank, and the total norm (reference DASolver.C:745-1000).

@@ -154,7 +154,10 @@ int dab_get_of_field(dab_solver* s, const char* name, const char* type, double* 
 int dab_get_residuals(dab_solver* s, int is_pc, double* residuals);
 
 /* calcJacTVecProduct(inputName, inputType, input, outputName, outputType, seed, product)
- * (reference DASolver.C:1690-1839).  Supported pairs: (stateVar -> residual), (stateVar -> function). */
+ * (reference DASolver.C:1690-1839).  Supported pairs: (stateVar -> residual), (stateVar -> function),
+ * (stateVar -> forceCouplingOutput), (volCoord -> forceCouplingOutput), and patchVelocity / patchVar /
+ * fvSourcePar / volCoord -> residual and function.  A forceCouplingOutput seed has dab_get_output_size
+ * entries (this rank's nodes). */
 int dab_calc_jac_t_vec_product(dab_solver* s, const char* input_name, const char* input_type, const double* input,
                                const char* output_name, const char* output_type, const double* seed,
                                double* product);
@@ -232,6 +235,17 @@ int dab_calc_function(dab_solver* s, const char* name, double* value);
 /* getInputSize / getOutputSize (pyDASolvers.pyx:189-199) */
 int dab_get_input_size(dab_solver* s, const char* name, const char* type, int64_t* out);
 int dab_get_output_size(dab_solver* s, const char* name, const char* type, int64_t* out);
+
+/* calcOutput(name, type, out) for type forceCouplingOutput (reference DAOutputForceCoupling.C:19-215): the wall force
+ * Sf (p_b - pRef) + Sf & devRhoReff_b of every face of the output's patches split equally over the face's points;
+ * out[3 * n + k] is component k on output node n.  The patches follow their names in sorted order; each patch lists
+ * its points (this rank's faces only) in ascending label order, so a point shared by two patches appears once per
+ * patch.  3 * nodes entries, possibly none. */
+int dab_calc_output(dab_solver* s, const char* name, const char* type, double* out);
+
+/* The global point index of every node of a forceCouplingOutput, in output order (dab_get_output_size / 3
+ * entries).  On several ranks a point on a partition seam is a node of each rank that has faces around it. */
+int dab_get_output_points(dab_solver* s, const char* name, int64_t* labels);
 
 /* --- benchmarking hooks (no reference counterpart): run the product n times on device-resident
  * vectors and return the mean device time per launch sequence in milliseconds (CUDA events on the
