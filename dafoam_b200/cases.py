@@ -602,7 +602,8 @@ def write_field(case_dir, name, cls, dims, internal, bcs, time="0"):
 
 def write_dicts(case_dir, nu=1.5e-5, ras_model="SpalartAllmaras", div_u="bounded Gauss linearUpwind grad(U)",
                 div_nut="bounded Gauss upwind", relax_u=0.7, relax_p=0.3, relax_nut=0.7, consistent=False, transonic=False,
-                div_phid_p="Gauss upwind"):
+                div_phid_p="Gauss upwind", relax_p_eqn=None, relax_he=None):
+    """relax_p_eqn: relaxationFactors.equations.p (pEqn.relax() of the transonic corrector); relax_he: equations e and h."""
     os.makedirs(os.path.join(case_dir, "constant"), exist_ok=True)
     os.makedirs(os.path.join(case_dir, "system"), exist_ok=True)
     with open(os.path.join(case_dir, "constant", "transportProperties"), "w") as f:
@@ -642,9 +643,10 @@ SIMPLE
 relaxationFactors
 {
     fields { p %.17g; }
-    equations { U %.17g; nuTilda %.17g; }
+    equations { U %.17g; nuTilda %.17g;%s }
 }
-""" % ("true" if consistent else "false", "yes" if transonic else "no", relax_p, relax_u, relax_nut))
+""" % ("true" if consistent else "false", "yes" if transonic else "no", relax_p, relax_u, relax_nut,
+       ("" if relax_p_eqn is None else " p %.17g;" % relax_p_eqn) + ("" if relax_he is None else " e %.17g; h %.17g;" % (relax_he, relax_he))))
     with open(os.path.join(case_dir, "system", "controlDict"), "w") as f:
         f.write(_header("dictionary", "system", "controlDict"))
         f.write("\napplication simpleFoam;\nstartTime 0;\nendTime 1000;\ndeltaT 1;\n")

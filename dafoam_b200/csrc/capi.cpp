@@ -520,6 +520,37 @@ int dab_get_face_loop_width(dab_solver* s, int* nf)
     DAB_CATCH
 }
 
+int dab_transonic_pressure_probe(dab_solver* s, int coarse, int* max_cf, int* n_agg, int32_t* nbr, double* off, double* diag, double* b,
+                                 double* x, int* iterations, int32_t* agg_of, const double* rc, double* yc)
+{
+    DAB_TRY
+    need(s, "solver");
+    need(max_cf, "max_cf");
+    need(n_agg, "n_agg");
+    Solver& S = s->s;
+    S.primalSetup();
+    *max_cf = S.hm.maxCF;
+    *n_agg = S.primal.nAgg;
+    if (!off) return 0;
+    need(nbr, "nbr");
+    need(diag, "diag");
+    need(b, "b");
+    need(x, "x");
+    need(iterations, "iterations");
+    need(agg_of, "agg_of");
+    std::vector<double> o, d, bb, xx;
+    std::vector<int32_t> a;
+    S.transonicPressureProbe(coarse, o, d, bb, xx, *iterations, a, rc, yc);
+    const size_t nC = (size_t)S.hm.nC;
+    for (size_t i = 0; i < (size_t)S.hm.maxCF * nC; i++) nbr[i] = S.hm.cellNbr[i] < (int)nC ? S.hm.cellNbr[i] : -1;
+    std::copy(o.begin(), o.end(), off);
+    std::copy(d.begin(), d.end(), diag);
+    std::copy(bb.begin(), bb.end(), b);
+    std::copy(xx.begin(), xx.end(), x);
+    std::copy(a.begin(), a.end(), agg_of);
+    DAB_CATCH
+}
+
 int dab_calc_pc_mat_fvmatrix(dab_solver* s, int turb_only, int64_t* nnz, int32_t* rows, int32_t* cols, double* vals)
 {
     DAB_TRY

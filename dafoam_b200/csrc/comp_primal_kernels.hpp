@@ -454,6 +454,172 @@ struct cPhiUpdate
     }
 };
 
+// rho = thermo.rho() = psi p, bounded (DAUtility::boundVar); the transonic corrector does not relax it (pEqnTurbo.H:1-8)
+struct RhoThermo
+{
+    Params q;
+    StateView s;
+    double* rho;
+    double lo, hi;
+    DAB_HD void operator()(int c) const
+    {
+        const double rn = s.p[c] * frcp(q.Rg * s.T[c]);
+        rho[c] = rn < lo ? lo : (rn > hi ? hi : rn);
+    }
+};
+
+// div(phid,p) face weight of the owner's p: the transonic branch of cFaceF, evaluated on the current p (the limiter is frozen in
+// the matrix, as fvm::div does)
+DAB_HD double cPhidWeight(const MeshView& m, const Params& q, const StateView& s, const RecordView& r, double phid, int f, int o, int n)
+{
+    const double w = m.w[f];
+    if (q.divPhidP == DIV_LINEAR) return w;
+    if (q.divPhidP == DIV_LIMITED_LINEAR)
+    {
+        double dl, gf, gc;
+        bool fb;
+        const double lim = limitedLinearLimiter(m, s, r, q.phidK, phid > 0.0, o, n, dl, gf, gc, fb);
+        return lim * w + (1.0 - lim) * (phid >= 0.0 ? 1.0 : 0.0);
+    }
+    return phid >= 0.0 ? 1.0 : 0.0;
+}
+
+// phid = psi_f (S_f.HbyA_f - relative-frame flux) and gam = (rho rAU)_f of an internal face: the same arithmetic as cFaceF
+DAB_HD void cPhidFace(const MeshView& m, const Params& q, const StateView& s, const RecordView& r, int f, int o, int n, double& phid,
+                      double& gam, double& cg)
+{
+    const int nT = m.nCtot;
+    const double w = m.w[f];
+    double ph = 0.0;
+    cg = 0.0;
+    const double Sv[3] = {m.Sx[f], m.Sy[f], m.Sz[f]};
+    const double kv[3] = {m.kx[f], m.ky[f], m.kz[f]};
+    for (int j = 0; j < 3; j++)
+    {
+        ph += Sv[j] * (w * r.HbyA[(size_t)j * nT + o] + (1.0 - w) * r.HbyA[(size_t)j * nT + n]);
+        cg += kv[j] * (w * r.gP[(size_t)j * nT + o] + (1.0 - w) * r.gP[(size_t)j * nT + n]);
+    }
+    gam = w * r.rho[o] * r.rAU[o] + (1.0 - w) * r.rho[n] * r.rAU[n];
+    if (m.mrfFlux) ph -= m.mrfFlux[f];
+    phid = (w * frcp(q.Rg * s.T[o]) + (1.0 - w) * frcp(q.Rg * s.T[n])) * ph;
+}
+
+// transonic pressure equation (pEqnTurbo.H transonic branch): fvm::div(phid, p) - fvm::laplacian(rho rAU, p) with an explicit
+// non-orthogonal correction, row c = sum over its faces of s_f F_f, F_f the transonic face flux of cFaceF.  Boundary faces:
+// F_b = psi_b p_b ph - rho_b rAU_c |S_f| snGrad(p)_b with p_b, snGrad(p)_b linear in p_c through bcScalar.  Not symmetric.
+// pEqn.relax() (relaxationFactors.equations.p) when alphaEqn > 0, with the scalar fvMatrix::relax rule of cEEqnAssemble.
+// face[] records what pEqn.flux() needs from the assembly: the owner's div(phid,p) weight of internal faces, rho_b of boundary faces.
+template <int NF>
+struct cPEqnTransonic
+{
+    MeshView m;
+    Params q;
+    StateView s;
+    RecordView r;
+    EqnView e;
+    double alphaEqn;
+    double* face; // [nF]
+    DAB_HD void operator()(int c) const
+    {
+        const int nC = e.nC;
+        double D0 = 0.0, sumOff = 0.0, B = 0.0, ic = 0.0, aic = 0.0;
+        for (int k = 0; k < m.maxCF; k++)
+        {
+            const FaceRef fr = faceOf(m, c, k);
+            if (fr.f < 0)
+            {
+                for (int kk = k; kk < m.maxCF; kk++) e.off[(size_t)kk * nC + c] = 0.0;
+                break;
+            }
+            const int f = fr.f;
+            const double mS = m.magSf[f], dl = m.delta[f];
+            if (!fr.bnd)
+            {
+                const int o = fr.s > 0 ? c : fr.n, n = fr.s > 0 ? fr.n : c;
+                double phid, gam, cg;
+                cPhidFace(m, q, s, r, f, o, n, phid, gam, cg);
+                const double wf = cPhidWeight(m, q, s, r, phid, f, o, n);
+                if (fr.s > 0) face[f] = wf;
+                const double wc = fr.s > 0 ? wf : 1.0 - wf;
+                const double mphid = fr.s * phid, g = gam * mS * dl;
+                const double off = mphid * (1.0 - wc) - g;
+                e.off[(size_t)k * nC + c] = off;
+                D0 += mphid * wc + g;
+                sumOff += fabs(off);
+                B += fr.s * gam * mS * cg;
+            }
+            else
+            {
+                e.off[(size_t)k * nC + c] = 0.0;
+                BoundaryPoint bp;
+                boundaryPoint<false>(m, q, s, r, f, c, bp);
+                face[f] = bp.th.rho;
+                const double pRef = q.bcVal[F_P][m.bPatch[f - m.nIF]][0];
+                const double cv = frcp(q.Rg * bp.T) * cPhBoundary(m, q, r, bp, f, c); // psi_b ph
+                const double gb = bp.th.rho * r.rAU[c] * mS * dl * bp.frP;
+                const double icf = cv * (1.0 - bp.frP) + gb;
+                ic += icf;
+                aic += fabs(icf);
+                B -= (cv - gb) * bp.frP * pRef;
+            }
+        }
+        if (alphaEqn > 0.0)
+        {
+            const double D1 = D0 + aic;
+            const double aD1 = fabs(D1);
+            const double D2 = aD1 > sumOff ? aD1 : sumOff;
+            const double Dn = D2 * frcp(alphaEqn) - ic;
+            e.diag[c] = Dn + ic;
+            e.b[c] = B + (Dn - D0) * s.p[c];
+        }
+        else
+        {
+            e.diag[c] = D0 + ic;
+            e.b[c] = B;
+        }
+        (void)NF;
+    }
+};
+
+// phi == pEqn.flux() of the transonic corrector: F_f of the matrix at the solved p, with the div(phid,p) weights and rho_b frozen at
+// assembly and the non-orthogonal correction of the assembly's grad(p).  At the fixed point this is the residual's F (cFaceF, cFwdC).
+template <int NF>
+struct cPhiTransonic
+{
+    MeshView m;
+    Params q;
+    StateView s;
+    RecordView r;
+    const double* face; // cPEqnTransonic's record
+    double* phi;
+    DAB_HD void operator()(int c) const
+    {
+        for (int k = 0; k < m.maxCF; k++)
+        {
+            const FaceRef fr = faceOf(m, c, k);
+            if (fr.f < 0) break;
+            if (fr.s < 0) continue;
+            const int f = fr.f;
+            if (!fr.bnd)
+            {
+                const int n = fr.n;
+                double phid, gam, cg;
+                cPhidFace(m, q, s, r, f, c, n, phid, gam, cg);
+                const double wf = face[f];
+                phi[f] = phid * (wf * s.p[c] + (1.0 - wf) * s.p[n]) - gam * m.magSf[f] * (m.delta[f] * (s.p[n] - s.p[c]) + cg);
+            }
+            else
+            {
+                BoundaryPoint bp;
+                boundaryPoint<false>(m, q, s, r, f, c, bp);
+                const double cv = frcp(q.Rg * bp.T) * cPhBoundary(m, q, r, bp, f, c);
+                phi[f] = cv * bp.p - face[f] * r.rAU[c] * m.magSf[f] * bp.sngP;
+            }
+        }
+        (void)NF;
+    }
+};
+
 // nuTilda equation, compressible form (DASpalartAllmaras.C:452-462 with rho)
 template <int NF>
 struct cNutEqnAssemble

@@ -782,6 +782,17 @@ struct CoarseApply // yc = Ainv rc (Ainv symmetric: column access is coalesced)
         yc[i] = s;
     }
 };
+struct TransposeSq // At = A^T (n x n): a nonsymmetric inverse read by CoarseApply's coalesced column access
+{
+    const double* A;
+    int n;
+    double* At;
+    DAB_HD void operator()(int t) const
+    {
+        const int i = t / n, j = t - i * n;
+        At[(size_t)j * n + i] = A[t];
+    }
+};
 struct CoarseProlongAdd // z[c] += yc[agg[c]]
 {
     const double* yc;
@@ -805,6 +816,97 @@ struct ResidualOf // r = b - q
     const double *b, *q;
     double* r;
     DAB_HD void operator()(int c) const { r[c] = b[c] - q[c]; }
+};
+
+// ---- BiCGStab (van der Vorst) for the nonsymmetric transonic pressure equation, scalars on the device:
+// S[0] rho = (rhat, r), S[1] rho of the previous iteration, S[2] alpha, S[3] omega, S[4] beta, S[5] (rhat, v), S[6] (t, s), S[7] (t, t),
+// S[8] sum |r|, S[9] breakdown flag (rho, (rhat, v) or (t, t) vanished): once set, alpha = omega = 0 leave x alone until the host
+// restarts from the true residual
+constexpr double BICG_VSMALL = 1e-300;
+struct BicgBeta
+{
+    double* S;
+    int first;
+    DAB_HD void operator()(int) const
+    {
+        if (!(fabs(S[0]) > BICG_VSMALL)) S[9] = 1.0;
+        S[4] = (first || S[9] != 0.0) ? 0.0 : (S[0] / S[1]) * (S[2] / S[3]);
+        S[1] = S[0];
+    }
+};
+struct BicgAlpha
+{
+    double* S;
+    DAB_HD void operator()(int) const
+    {
+        if (!(fabs(S[5]) > BICG_VSMALL)) S[9] = 1.0;
+        S[2] = S[9] != 0.0 ? 0.0 : S[0] / S[5];
+    }
+};
+struct BicgOmega
+{
+    double* S;
+    DAB_HD void operator()(int) const
+    {
+        if (!(S[7] > BICG_VSMALL)) S[9] = 1.0;
+        S[3] = S[9] != 0.0 ? 0.0 : S[6] / S[7];
+    }
+};
+struct BicgDir // p = r + beta (p - omega v)
+{
+    const double* S;
+    const double *r, *v;
+    double* p;
+    DAB_HD void operator()(int c) const
+    {
+        const double beta = S[4];
+        p[c] = beta == 0.0 ? r[c] : r[c] + beta * (p[c] - S[3] * v[c]);
+    }
+};
+struct BicgHalf // x += alpha y; s = r - alpha v (in r)
+{
+    const double* S;
+    const double *y, *v;
+    double *x, *r;
+    DAB_HD void operator()(int c) const
+    {
+        const double a = S[2];
+        x[c] += a * y[c];
+        r[c] -= a * v[c];
+    }
+};
+struct BicgFull // x += omega z; r = s - omega t; absr = |r|
+{
+    const double* S;
+    const double *z, *t;
+    double *x, *r, *absr;
+    DAB_HD void operator()(int c) const
+    {
+        const double w = S[3];
+        x[c] += w * z[c];
+        const double v = r[c] - w * t[c];
+        r[c] = v;
+        absr[c] = fabs(v);
+    }
+};
+struct SpmvEllDot2 // t = A z, out0 = t*s, out1 = t*t
+{
+    EqnView e;
+    const double *z, *s;
+    double *t, *out0, *out1;
+    DAB_HD void operator()(int c) const
+    {
+        const int nC = e.nC;
+        double acc = e.diag[c] * z[c];
+        for (int k = 0; k < e.maxCF; k++)
+        {
+            const int n = e.cellNbr[(size_t)k * nC + c];
+            if (n >= 0) acc += e.off[(size_t)k * nC + c] * z[n];
+        }
+        t[c] = acc;
+        out0[c] = acc * s[c];
+        out1[c] = acc * acc;
+    }
 };
 struct FillConst
 {
@@ -837,9 +939,12 @@ struct Primal
     SegControl cU, cP, cN, cE;
     double ntMin = 1e-16, ntMax = 1e16;
     double pMin = 20000.0, pMax = 500000.0, TMin = 100.0, TMax = 1000.0, UMax = 1000.0; // DAOption primalVarBounds (compressible)
+    double rhoMin = 0.2, rhoMax = 5.0;
+    double alphaPEqn = 0.0; // relaxationFactors.equations.p of the transonic pressure equation; 0: not relaxed
     bool allocated = false;
     DevBuf<double> uOff, uDiag, uB, pOff, pDiag, pB, nOff, nDiag, nB;
     DevBuf<double> Utmp, pOld, ntTmp, red, ones, r, z, d, q, eOff, eDiag, eB, heTmp, rAt, gPOld;
+    DevBuf<double> pFace, bRhat, bDir, bV, bT, dAcT; // transonic corrector: assembly record, BiCGStab vectors, transposed coarse inverse
     DevBuf<int32_t> dColourOf, dColourList;
     std::vector<int> colourStart; // [nColours+1] into dColourList
     // pressure coarse space

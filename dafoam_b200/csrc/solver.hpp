@@ -587,6 +587,7 @@ struct Solver
             if (rf.hasSub("equations")) primal.alphaN = rf.sub("equations").scalarOr("nuTilda", primal.alphaN);
             if (rf.hasSub("equations"))
                 primal.alphaE = rf.sub("equations").scalarOr("e", rf.sub("equations").scalarOr("h", primal.alphaE));
+            if (rf.hasSub("equations")) primal.alphaPEqn = rf.sub("equations").scalarOr("p", 0.0); // pEqn.relax(): transonic only
         }
         if (fso.hasSub("SIMPLE")) primal.nNonOrth = (int)fso.sub("SIMPLE").scalarOr("nNonOrthogonalCorrectors", 0.0);
         if (fso.hasSub("solvers"))
@@ -748,6 +749,8 @@ struct Solver
             primal.TMin = vb->numOr("TMin", primal.TMin);
             primal.TMax = vb->numOr("TMax", primal.TMax);
             primal.UMax = vb->numOr("UMax", primal.UMax);
+            primal.rhoMin = vb->numOr("rhoMin", primal.rhoMin);
+            primal.rhoMax = vb->numOr("rhoMax", primal.rhoMax);
         }
         adjPCLag = (int)o.numOr("adjPCLag", (double)adjPCLag);
         if (const JVal* wj = o.get("writeJacobians"))
@@ -2565,9 +2568,12 @@ struct Solver
     void primalResidual(const EqnView& e, const double* x, const double* g, double* res);
     void primalJacobi(const EqnView& e, double* x, double* tmp, const double* g, const SegControl& ctl, double* res0);
     void primalCoarseSetup();
-    void primalCoarseRefresh(const EqnView& e);
-    void primalPrecond(const EqnView& e, const double* r, double* z);
+    void primalCoarseRefresh(const EqnView& e, bool nonsym = false);
+    void primalPrecond(const EqnView& e, const double* r, double* z, bool nonsym = false);
     int primalPcg(const EqnView& e, double* x, const SegControl& ctl, double& res0);
+    int primalBicgstab(const EqnView& e, double* x, const SegControl& ctl, double& res0);
+    void transonicPressureProbe(int coarse, std::vector<double>& off, std::vector<double>& diag, std::vector<double>& b, std::vector<double>& x,
+                                int& iters, std::vector<int32_t>& aggOf, const double* rc, double* yc);
     int solvePrimal(PrimalStats& st);
 
     // ---- Krylov -----------------------------------------------------------------------------------

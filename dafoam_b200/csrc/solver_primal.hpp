@@ -60,7 +60,7 @@ inline void Solver::primalSetup()
     }
     P.dColourOf.upload(be, colourOf);
     P.dColourList.upload(be, list);
-    P.dS.alloc(be, 8);
+    P.dS.alloc(be, 16); // PCG: S[0..5], BiCGStab: S[0..9]
     primalCoarseSetup();
     P.allocated = true;
 }
@@ -169,7 +169,7 @@ inline void Solver::primalCoarseSetup()
 }
 
 // Galerkin coarse operator of the current pressure matrix and its inverse (device, Gauss-Jordan)
-inline void Solver::primalCoarseRefresh(const EqnView& e)
+inline void Solver::primalCoarseRefresh(const EqnView& e, bool nonsym)
 {
     Primal& P = primal;
     if (P.nAgg == 0) return;
@@ -181,11 +181,17 @@ inline void Solver::primalCoarseRefresh(const EqnView& e)
         be.launch(n, GjStep1{P.dAc.p, P.dColk.p, n, k});
         be.launch(n * n, GjStep2{P.dAc.p, P.dColk.p, n, k});
     }
+    if (nonsym)
+    {
+        // CoarseApply reads columns; the inverse of a nonsymmetric Galerkin operator is read through its transpose
+        if (!P.dAcT.p) P.dAcT.alloc(be, (size_t)n * n);
+        be.launch(n * n, TransposeSq{P.dAc.p, n, P.dAcT.p});
+    }
     P.coarseValid = true;
 }
 
 // z = M^{-1} r: multicolour symmetric Gauss-Seidel, M = (D+L) D^{-1} (D+U), plus the additive coarse correction
-inline void Solver::primalPrecond(const EqnView& e, const double* r, double* z)
+inline void Solver::primalPrecond(const EqnView& e, const double* r, double* z, bool nonsym)
 {
     const Primal& P = primal;
     const int nCol = (int)P.colourStart.size() - 1;
@@ -199,7 +205,7 @@ inline void Solver::primalPrecond(const EqnView& e, const double* r, double* z)
     {
         be.launch(P.nChunks, CoarseRestrict1{r, P.dAggCells.p, P.dChunkStart.p, P.dPartial.p});
         be.launch(P.nAgg, CoarseRestrict2{P.dPartial.p, P.dAggChunkOff.p, P.dRc.p});
-        be.launch(P.nAgg, CoarseApply{P.dAc.p, P.dRc.p, P.nAgg, P.dYc.p});
+        be.launch(P.nAgg, CoarseApply{nonsym ? P.dAcT.p : P.dAc.p, P.dRc.p, P.nAgg, P.dYc.p});
         be.launch(hm.nC, CoarseProlongAdd{P.dYc.p, P.dAggOf.p, z});
     }
 }
@@ -250,11 +256,165 @@ inline int Solver::primalPcg(const EqnView& e, double* x, const SegControl& ctl,
     return it;
 }
 
+// Preconditioned BiCGStab (van der Vorst 1992) on the nonsymmetric transonic pressure equation: the preconditioner of primalPcg
+// (multicolour symmetric Gauss-Seidel on the matrix rows + the additive coarse space through the transposed coarse inverse), the same
+// OpenFOAM-normalised residual and solvers.p controls, scalars on the device and the residual read by the host every few iterations.
+// A breakdown ((rhat, r), (rhat, v) or (t, t) vanishing) freezes x until the next check, which restarts from the true residual;
+// the iteration count stays bounded by maxIter either way.
+inline int Solver::primalBicgstab(const EqnView& e, double* x, const SegControl& ctl, double& res0)
+{
+    Primal& P = primal;
+    const int nC = hm.nC, nT = hm.nCtot;
+    if (!P.bRhat.p)
+    {
+        P.bRhat.alloc(be, nC); P.bDir.alloc(be, nC); P.bV.alloc(be, nC); P.bT.alloc(be, nC);
+    }
+    double r1[3];
+    primalResidual(e, x, nullptr, r1);
+    res0 = r1[0];
+    if (res0 < ctl.tol) return 0;
+    double* S = P.dS.p;
+    double* y = P.z.p; // M^-1 p and M^-1 s carry ghost copies for the products
+    double* z = P.d.p;
+    double normFactor = 0.0;
+    const int checkEvery = 4;
+    int it = 0, restarts = 0;
+    bool first = true;
+    while (it < ctl.maxIter)
+    {
+        if (first)
+        {
+            // r = b - A x, rhat = r
+            if (ghosted()) halo.exchangeCells({{x, 1, 1, nT}});
+            be.launch(nC, SpmvEll{e, x, P.q.p});
+            be.launch(nC, ResidualOf{e.b, P.q.p, P.r.p});
+            be.d2d(P.bRhat.p, P.r.p, (size_t)nC * sizeof(double));
+            be.zero(S, 10 * sizeof(double));
+            if (normFactor == 0.0)
+            {
+                // norm factor once (OpenFOAM keeps it fixed during the solve)
+                be.launch(nC, PcgProducts{P.r.p, P.r.p, P.r.p, P.red.p, P.red.p + nC});
+                normFactor = primalSums(2)[1] / res0;
+            }
+        }
+        be.launch(nC, PcgProducts{P.bRhat.p, P.r.p, P.r.p, P.red.p, nullptr});
+        P.ops->dotsDev(P.red.p, nC, 1, P.ones.p, nC, S + 0);
+        be.launch(1, BicgBeta{S, first ? 1 : 0});
+        first = false;
+        be.launch(nC, BicgDir{S, P.r.p, P.bV.p, P.bDir.p});
+        primalPrecond(e, P.bDir.p, y, true);
+        if (ghosted()) halo.exchangeCells({{y, 1, 1, nT}});
+        be.launch(nC, SpmvEllProd{e, y, P.bV.p, P.red.p});
+        be.launch(nC, PcgProducts{P.bRhat.p, P.bV.p, P.r.p, P.red.p, nullptr});
+        P.ops->dotsDev(P.red.p, nC, 1, P.ones.p, nC, S + 5);
+        be.launch(1, BicgAlpha{S});
+        be.launch(nC, BicgHalf{S, y, P.bV.p, x, P.r.p});
+        primalPrecond(e, P.r.p, z, true);
+        if (ghosted()) halo.exchangeCells({{z, 1, 1, nT}});
+        be.launch(nC, SpmvEllDot2{e, z, P.r.p, P.bT.p, P.red.p, P.red.p + nC});
+        P.ops->dotsDev(P.red.p, nC, 2, P.ones.p, nC, S + 6);
+        be.launch(1, BicgOmega{S});
+        be.launch(nC, BicgFull{S, z, P.bT.p, x, P.r.p, P.red.p});
+        P.ops->dotsDev(P.red.p, nC, 1, P.ones.p, nC, S + 8);
+        it++;
+        if (it % checkEvery == 0 || it == ctl.maxIter)
+        {
+            double h[2];
+            be.d2h(h, S + 8, 2 * sizeof(double));
+            if (!(h[0] == h[0])) throw Error("pressure solver diverged (NaN)");
+            if (h[1] != 0.0)
+            {
+                // breakdown: restart from the true residual (more than three restarts in one solve are a failure)
+                if (++restarts > 3)
+                {
+                    double sv[10];
+                    be.d2h(sv, S, sizeof(sv));
+                    char msg[256];
+                    snprintf(msg, sizeof(msg), "pressure solver: BiCGStab broke down repeatedly (iteration %d: (rhat, r) = %.3e, (rhat, v) = %.3e, "
+                             "(t, t) = %.3e)", it, sv[0], sv[5], sv[7]);
+                    throw Error(msg);
+                }
+                first = true;
+                double rt[3];
+                primalResidual(e, x, nullptr, rt);
+                if (rt[0] < ctl.tol || rt[0] < ctl.relTol * res0) break;
+                continue;
+            }
+            const double res = h[0] / normFactor;
+            if (res < ctl.tol || res < ctl.relTol * res0) break;
+        }
+    }
+    return it;
+}
+
+// Test hook: the transonic pressure equation of the current state as the first SIMPLE iteration assembles it (momentum matrix and
+// HbyA of the current U, rho = psi p), its rows, right-hand side and one BiCGStab solve from the current p (the state is left as it
+// is); with the coarse space on, yc = Ac^-1 rc through the solver's own coarse apply.
+inline void Solver::transonicPressureProbe(int coarse, std::vector<double>& off, std::vector<double>& diag, std::vector<double>& b,
+                                           std::vector<double>& x, int& iters, std::vector<int32_t>& aggOf, const double* rc, double* yc)
+{
+    if (!par.transonic) throw Error("transonicPressureProbe: the case has no transonic pressure equation");
+    primalSetup();
+    if (fvSourceDirty) updateFvSource();
+    Primal& P = primal;
+    const int nC = hm.nC, nT = hm.nCtot, mcf = hm.maxCF;
+    if (!P.pFace.p) P.pFace.alloc(be, hm.nF);
+    EqnView eU{nC, mcf, 3, P.uOff.p, P.uDiag.p, P.uB.p, mv.cellNbr};
+    EqnView eP{nC, mcf, 1, P.pOff.p, P.pDiag.p, P.pB.p, mv.cellNbr};
+    const bool mr = ghosted();
+    auto exGrad = [&]() {
+        if (!mr) return;
+        std::vector<HaloItem> it{{rv.gU, 9, 1, nT}, {rv.gP, 3, 1, nT}, {rv.gHe, 3, 1, nT}};
+        if (par.turb) it.push_back({rv.gNt, 3, 1, nT});
+        halo.exchangeCells(it);
+    };
+    if (mr) exchangeStates();
+    Params pp = par;
+    pp.rhoFrozen = 1;
+    DAB_LAUNCH_NF(nT, cFwdA, mv, par, sv, rv);
+    exGrad();
+    DAB_LAUNCH_NF(nC, cUEqnAssemble, mv, pp, sv, rv, eU);
+    be.launch(nC, HbyAKernel{eU, sv, rv, mv.V, nT});
+    if (mr) halo.exchangeCells({{rv.rAU, 1, 1, nT}, {rv.HbyA, 3, 1, nT}});
+    DAB_LAUNCH_NF(nC, cPEqnTransonic, mv, par, sv, rv, eP, P.alphaPEqn, P.pFace.p);
+    primalCoarseRefresh(eP, true);
+    const bool coarseOn = coarse && P.nAgg > 0;
+    P.coarseValid = coarseOn;
+    off.resize((size_t)mcf * nC);
+    diag.resize(nC);
+    b.resize(nC);
+    x.resize(nC);
+    be.d2h(off.data(), P.pOff.p, off.size() * sizeof(double));
+    be.d2h(diag.data(), P.pDiag.p, diag.size() * sizeof(double));
+    be.d2h(b.data(), P.pB.p, b.size() * sizeof(double));
+    DevBuf<double> xd;
+    xd.alloc(be, nT);
+    be.d2d(xd.p, dP.p, (size_t)nT * sizeof(double));
+    double r0;
+    iters = primalBicgstab(eP, xd.p, P.cP, r0);
+    be.d2h(x.data(), xd.p, x.size() * sizeof(double));
+    aggOf.assign(nC, -1);
+    if (coarseOn)
+    {
+        be.d2h(aggOf.data(), P.dAggOf.p, (size_t)nC * sizeof(int32_t));
+        if (rc && yc)
+        {
+            be.h2d(P.dRc.p, rc, (size_t)P.nAgg * sizeof(double));
+            be.launch(P.nAgg, CoarseApply{P.dAcT.p, P.dRc.p, P.nAgg, P.dYc.p});
+            be.d2h(yc, P.dYc.p, (size_t)P.nAgg * sizeof(double));
+        }
+    }
+    be.sync();
+    P.coarseValid = false; // the next solvePrimal refreshes it at its first iteration
+    recorded = false;
+    kry.pcValid = false;
+}
+
 inline int Solver::solvePrimal(PrimalStats& st)
 {
-    if (par.transonic)
-        throw Error("solvePrimal: the transonic pressure corrector (pEqnRhoSimpleC.H / pEqnTurbo.H transonic branch, a non-symmetric "
-                    "convection-diffusion pressure equation) is not built; the residual, its transpose product and the adjoint solve are");
+    if (par.transonic && solverName != "DATurboFoam")
+        throw Error("solvePrimal: the transonic pressure corrector of " + solverName +
+                    " is not built (DATurboFoam's transonic branch of pEqnTurbo.H is); the residual, its transpose product and the adjoint solve are");
     primalSetup();
     if (fvSourceDirty) updateFvSource();
     Primal& P = primal;
@@ -310,6 +470,12 @@ inline int Solver::solvePrimal(PrimalStats& st)
             if (mr) halo.exchangeCells({{dT.p, 1, 1, nT}});
         }
         // pressure corrector
+        if (par.transonic)
+        {
+            // rho = thermo.rho(), bounded, not relaxed (pEqnTurbo.H:1-8)
+            be.launch(nC, RhoThermo{par, sv, rv.rho, P.rhoMin, P.rhoMax});
+            if (mr) halo.exchangeCells({{rv.rho, 1, 1, nT}});
+        }
         DAB_LAUNCH_NF(nT, cFwdA, mv, pp, sv, rv);
         exGrad();
         be.launch(nC, HbyAKernel{eU, sv, rv, mv.V, nT});
@@ -322,20 +488,46 @@ inline int Solver::solvePrimal(PrimalStats& st)
             be.d2d(P.gPOld.p, rv.gP, (size_t)3 * nT * sizeof(double));
             sc = Simplec{P.rAt.p, P.pOld.p, P.gPOld.p};
         }
-        DAB_LAUNCH_NF(nC, cPEqnAssemble, mv, pp, sv, rv, eP, sc);
-        if (it == 1 || (it - 1) % P.coarseRefresh == 0) primalCoarseRefresh(eP);
+        if (par.transonic)
         {
-            double rp;
-            st.pIterations += primalPcg(eP, dP.p, P.cP, rp);
-            st.resP = rp;
-            maxRes = std::max(maxRes, rp);
+            // DATurboFoam transonic branch (pEqnTurbo.H:22-55): fvm::div(phid, p) - fvm::laplacian(rho rAU, p), BiCGStab,
+            // phi == pEqn.flux() after the last non-orthogonal corrector; AtU enters only the velocity correction
+            if (!P.pFace.p) P.pFace.alloc(be, hm.nF);
+            for (int no = 0; no <= P.nNonOrth; no++)
+            {
+                if (no > 0)
+                {
+                    DAB_LAUNCH_NF(nT, cFwdA, mv, pp, sv, rv); // grad(p) of the latest p for the non-orthogonal correction
+                    exGrad();
+                }
+                DAB_LAUNCH_NF(nC, cPEqnTransonic, mv, par, sv, rv, eP, P.alphaPEqn, P.pFace.p);
+                if (no == 0 && (it == 1 || (it - 1) % P.coarseRefresh == 0 || !P.coarseValid)) primalCoarseRefresh(eP, true);
+                double rp;
+                st.pIterations += primalBicgstab(eP, dP.p, P.cP, rp);
+                if (no == 0) st.resP = rp;
+                maxRes = std::max(maxRes, rp);
+                if (mr) halo.exchangeCells({{dP.p, 1, 1, nT}});
+            }
+            DAB_LAUNCH_NF(nC, cPhiTransonic, mv, par, sv, rv, P.pFace.p, dPhi.p);
         }
-        if (mr) halo.exchangeCells({{dP.p, 1, 1, nT}});
-        DAB_LAUNCH_NF(nC, cPhiUpdate, mv, pp, sv, rv, dPhi.p, sc);
+        else
+        {
+            DAB_LAUNCH_NF(nC, cPEqnAssemble, mv, pp, sv, rv, eP, sc);
+            if (it == 1 || (it - 1) % P.coarseRefresh == 0) primalCoarseRefresh(eP);
+            {
+                double rp;
+                st.pIterations += primalPcg(eP, dP.p, P.cP, rp);
+                st.resP = rp;
+                maxRes = std::max(maxRes, rp);
+            }
+            if (mr) halo.exchangeCells({{dP.p, 1, 1, nT}});
+            DAB_LAUNCH_NF(nC, cPhiUpdate, mv, pp, sv, rv, dPhi.p, sc);
+        }
         if (mr) halo.exchangeFaces({{dPhi.p, 1, 1, hm.nF}});
         be.launch(nC, RelaxField{dP.p, P.pOld.p, P.alphaP});
         be.launch(nC, BoundField{dP.p, P.pMin, P.pMax});
-        be.launch(nC, RhoRelax{pp, sv, rv.rho, P.alphaRho});
+        if (par.transonic) be.launch(nC, RhoThermo{par, sv, rv.rho, P.rhoMin, P.rhoMax}); // after the velocity correction in
+        else be.launch(nC, RhoRelax{pp, sv, rv.rho, P.alphaRho});                       // pEqnTurbo.H, which does not read rho
         if (mr) halo.exchangeCells({{dP.p, 1, 1, nT}, {rv.rho, 1, 1, nT}});
         DAB_LAUNCH_NF(nT, cFwdA, mv, pp, sv, rv); // grad of the relaxed p, closures at the new (p, T)
         exGrad();

@@ -618,6 +618,31 @@ class pyDASolvers:
         self._raise(self._L.dab_get_face_loop_width(self._h, C.byref(nf)))
         return nf.value
 
+    def getTransonicPressureSystem(self, coarse=True, rc=None):
+        """Test hook: the transonic pressure equation of the current state (DATurboFoam, SIMPLE { transonic yes; }) as the first SIMPLE
+        iteration assembles it, and one BiCGStab solve of it from the current p; the states are not changed.  Returns a dict with the
+        ELL rows (nbr, off: [maxCF, nC]; diag, b: [nC]), the solution x, the iteration count, agg_of (local aggregate per cell, -1
+        without coarse space) and, when rc is given and the coarse space is on, yc = Ac^-1 rc from the solver's coarse apply."""
+        mcf, nagg = C.c_int(), C.c_int()
+        nil = None
+        self._raise(self._L.dab_transonic_pressure_probe(self._h, C.c_int(int(coarse)), C.byref(mcf), C.byref(nagg), nil, nil, nil, nil, nil,
+                                                         nil, nil, nil, nil))
+        nC = self.getNLocalCells()
+        ip = C.POINTER(C.c_int32)
+        nbr, off = np.zeros(mcf.value * nC, dtype=np.int32), np.zeros(mcf.value * nC)
+        diag, b, x, agg = np.zeros(nC), np.zeros(nC), np.zeros(nC), np.zeros(nC, dtype=np.int32)
+        its = C.c_int()
+        yc, rcp = None, None
+        if rc is not None:  # the first n_agg entries are used
+            assert len(rc) >= nagg.value, "rc needs n_agg = %d entries" % nagg.value
+            rc = np.ascontiguousarray(rc[:nagg.value], dtype=np.float64)
+            yc, rcp = np.zeros(nagg.value), _dp(rc)
+        self._raise(self._L.dab_transonic_pressure_probe(self._h, C.c_int(int(coarse)), C.byref(mcf), C.byref(nagg), nbr.ctypes.data_as(ip),
+                                                         _dp(off), _dp(diag), _dp(b), _dp(x), C.byref(its), agg.ctypes.data_as(ip), rcp,
+                                                         _dp(yc) if yc is not None else None))
+        return dict(nbr=nbr.reshape(mcf.value, nC), off=off.reshape(mcf.value, nC), diag=diag, b=b, x=x, iterations=its.value, agg_of=agg,
+                    n_agg=nagg.value, yc=yc)
+
     def initializedRdWTMatrixFree(self):
         return None
 

@@ -209,6 +209,16 @@ int dab_get_pc_aggregates(dab_solver* s, int32_t* agg_of);
  * rolled NF=0 loops). */
 int dab_get_face_loop_width(dab_solver* s, int* nf);
 
+/* Test hook (no counterpart in the reference): the transonic pressure equation of DATurboFoam (SIMPLE { transonic yes; }) at the
+ * current state as the first SIMPLE iteration assembles it (momentum matrix and HbyA of the current U, rho = psi p) and one
+ * BiCGStab solve of it from the current p; the states are not changed.  Rows: (diag[c] p_c + sum_k off[k*nC + c] p_nbr(k,c)) = b[c],
+ * nbr[k*nC + c] the neighbour of the k-th face of cell c (-1 for boundary faces and unused slots).
+ * coarse != 0 keeps the coarse space of the preconditioner; agg_of[c] is then the local aggregate of cell c (-1 without a coarse
+ * space) and, if rc and yc are given, yc = Ac^-1 rc (n_agg entries) through the solver's coarse apply.  off == NULL: only *max_cf
+ * and *n_agg are returned. */
+int dab_transonic_pressure_probe(dab_solver* s, int coarse, int* max_cf, int* n_agg, int32_t* nbr, double* off, double* diag, double* b,
+                                 double* x, int* iterations, int32_t* agg_of, const double* rc, double* yc);
+
 /* calcPCMatWithFvMatrix(PCMat, turbOnly) (reference pyDASolvers.pyx:99-114 list, DASolver.C:2888-2988): the turbulence block of
  * the preconditioner taken from the relaxed nuTilda fvMatrix (diag / lower / upper, `div(pc)` convection, DASpalartAllmaras.C:
  * 490-529), scaled and transposed like the reference, as COO triplets (row, column, value) in the local state numbering -- what the
