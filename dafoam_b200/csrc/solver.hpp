@@ -35,80 +35,6 @@
 namespace dab
 {
 
-// optional-feature dispatch for the two heavy kernels (hex meshes: 4 variants; other meshes: the full-featured one)
-#define DAB_LAUNCH_NFF(n, F, ...)                                     \
-    do                                                                \
-    {                                                                 \
-        if (hex6)                                            \
-        {                                                             \
-            switch (featureMask())                                    \
-            {                                                         \
-            case 0: be.launch(n, F<6, 0>{__VA_ARGS__}); break;        \
-            case 1: be.launch(n, F<6, 1>{__VA_ARGS__}); break;        \
-            case 2: be.launch(n, F<6, 2>{__VA_ARGS__}); break;        \
-            case 3: be.launch(n, F<6, 3>{__VA_ARGS__}); break;        \
-            default: be.launch(n, F<6, 7>{__VA_ARGS__}); break;       \
-            }                                                         \
-        }                                                             \
-        else be.launch(n, F<0, 7>{__VA_ARGS__});                      \
-    } while (0)
-
-// the same launches over the cell range [c0, c0 + n) (interior / cut-adjacent split for communication overlap)
-#define DAB_LAUNCH_NF_R(c0, n, F, ...)                                                      \
-    do                                                                                      \
-    {                                                                                       \
-        if (hex6) be.launch(n, Shifted<F<6>>{F<6>{__VA_ARGS__}, c0});              \
-        else be.launch(n, Shifted<F<0>>{F<0>{__VA_ARGS__}, c0});                            \
-    } while (0)
-#define DAB_LAUNCH_NFF_R(c0, n, F, ...)                                                     \
-    do                                                                                      \
-    {                                                                                       \
-        if (hex6)                                                                  \
-        {                                                                                   \
-            switch (featureMask())                                                          \
-            {                                                                               \
-            case 0: be.launch(n, Shifted<F<6, 0>>{F<6, 0>{__VA_ARGS__}, c0}); break;        \
-            case 1: be.launch(n, Shifted<F<6, 1>>{F<6, 1>{__VA_ARGS__}, c0}); break;        \
-            case 2: be.launch(n, Shifted<F<6, 2>>{F<6, 2>{__VA_ARGS__}, c0}); break;        \
-            case 3: be.launch(n, Shifted<F<6, 3>>{F<6, 3>{__VA_ARGS__}, c0}); break;        \
-            default: be.launch(n, Shifted<F<6, 7>>{F<6, 7>{__VA_ARGS__}, c0}); break;       \
-            }                                                                               \
-        }                                                                                   \
-        else be.launch(n, Shifted<F<0, 7>>{F<0, 7>{__VA_ARGS__}, c0});                      \
-    } while (0)
-
-// hexahedral meshes (6 faces per cell) get fully unrolled face loops; anything else the run-time loop
-#define DAB_LAUNCH_NF(n, F, ...)                                  \
-    do                                                            \
-    {                                                             \
-        if (hex6) be.launch(n, F<6>{__VA_ARGS__});       \
-        else be.launch(n, F<0>{__VA_ARGS__});                     \
-    } while (0)
-
-// the same with an L2 prefetch plan (backend.hpp PfPlan)
-#define DAB_LAUNCH_NF_PF(pl, n, F, ...)                           \
-    do                                                            \
-    {                                                             \
-        if (hex6) be.launchPf(n, F<6>{__VA_ARGS__}, pl);          \
-        else be.launchPf(n, F<0>{__VA_ARGS__}, pl);               \
-    } while (0)
-#define DAB_LAUNCH_NFF_PF(pl, n, F, ...)                                  \
-    do                                                                    \
-    {                                                                     \
-        if (hex6)                                                         \
-        {                                                                 \
-            switch (featureMask())                                        \
-            {                                                             \
-            case 0: be.launchPf(n, F<6, 0>{__VA_ARGS__}, pl); break;      \
-            case 1: be.launchPf(n, F<6, 1>{__VA_ARGS__}, pl); break;      \
-            case 2: be.launchPf(n, F<6, 2>{__VA_ARGS__}, pl); break;      \
-            case 3: be.launchPf(n, F<6, 3>{__VA_ARGS__}, pl); break;      \
-            default: be.launchPf(n, F<6, 7>{__VA_ARGS__}, pl); break;     \
-            }                                                             \
-        }                                                                 \
-        else be.launchPf(n, F<0, 7>{__VA_ARGS__}, pl);                    \
-    } while (0)
-
 // DAInputPatchVelocity (reference src/adjoint/DAInput/DAInputPatchVelocity.C): input = (|U|, angle of attack in degrees)
 struct PatchVelocityDef
 {
@@ -283,6 +209,58 @@ struct Solver
                 if (par.bcKind[F_NUT][p] == BC_NUT_SPALDING) f |= 2;
         if (av.bcRefb) f = 7; // patchVelocity product: the full-featured variant also carries the BC-reference adjoint
         return f;
+    }
+
+    // the template instance of a kernel: hexahedral meshes (6 faces per cell) get fully unrolled face loops, NF = 6, anything else
+    // the run-time loop, NF = 0.  The heavy kernels also take an optional-feature variant FEAT: featureMask() where it is 0-3 on a
+    // hexahedral mesh, else the full-featured FULL (7 for the cell-per-thread kernels, 3 for the tile kernels)
+    template <int N>
+    using Int = std::integral_constant<int, N>;
+    template <class L>
+    void withNF(L&& l) const
+    {
+        if (hex6) l(Int<6>());
+        else l(Int<0>());
+    }
+    template <int FULL, class L>
+    void withNFF(L&& l) const
+    {
+        if (!hex6) return l(Int<0>(), Int<FULL>());
+        switch (featureMask())
+        {
+        case 0: l(Int<6>(), Int<0>()); break;
+        case 1: l(Int<6>(), Int<1>()); break;
+        case 2: l(Int<6>(), Int<2>()); break;
+        case 3: l(Int<6>(), Int<3>()); break;
+        default: l(Int<6>(), Int<FULL>()); break;
+        }
+    }
+
+    // a cell-per-thread launch over the cells [0, n) is kernel1d<K>.  Cells{n, c0} runs K over the range [c0, c0 + n) as
+    // kernel1d<Shifted<K>>, a kernel of its own (the interior / cut-adjacent split of the several-rank product); Cells{n, -1, pl}
+    // runs it over [0, n) through be.launchPf with the L2 prefetch plan pl (kernel1d<K> while the plan is off)
+    struct Cells
+    {
+        int n, c0 = -1;
+        PfPlan pl{};
+    };
+    template <class F>
+    void launchOn(int n, const F& f) { be.launch(n, f); }
+    template <class F>
+    void launchOn(const Cells& at, const F& f)
+    {
+        if (at.c0 >= 0) be.launch(at.n, Shifted<F>{f, at.c0});
+        else be.launchPf(at.n, f, at.pl);
+    }
+    template <template <int> class K, class At, class... A>
+    void launchNF(const At& at, const A&... a)
+    {
+        withNF([&](auto nf) { launchOn(at, K<nf>{a...}); });
+    }
+    template <template <int, int> class K, class At, class... A>
+    void launchNFF(const At& at, const A&... a)
+    {
+        withNFF<7>([&](auto nf, auto ft) { launchOn(at, K<nf, ft>{a...}); });
     }
 
     // ------------------------------------------------------------------------------------------
@@ -1215,6 +1193,7 @@ struct Solver
         // the plans do not make the product faster -- they stay an opt-in measurement hook (DAB_PREFETCH_L2=1), not the default
         const char* env = getenv("DAB_PREFETCH_L2");
         if (!env || atoi(env) == 0) return;
+        if (partitioned) return; // the product on a ghosted mesh runs cell ranges without plans (matVecDev)
         const int nC = hm.nC, nIF = hm.nIF;
         for (int f = 1; f < nIF; f++)
             if (hm.own[f] < hm.own[f - 1]) return; // not in upper-triangular order: no plan
@@ -1342,7 +1321,7 @@ struct Solver
         EqnView e{nC, mcf, 1, off.p, diag.p, b.p, mv.cellNbr};
         Params pq = par;
         pq.divNut = DIV_UPWIND; // "div(pc)"
-        DAB_LAUNCH_NF(nC, NutEqnAssemble, mv, pq, sv, rv, e, primal.alphaN);
+        launchNF<NutEqnAssemble>(nC, mv, pq, sv, rv, e, primal.alphaN);
         std::vector<double> hOff((size_t)mcf * nC), hD(nC);
         be.d2h(hOff.data(), off.p, hOff.size() * sizeof(double));
         be.d2h(hD.data(), diag.p, hD.size() * sizeof(double));
@@ -1373,22 +1352,11 @@ struct Solver
     bool tileProduct() const { return tilesOn && av.bcRefb == nullptr; }
     void launchTileA(const PsiView& pv)
     {
-        if (hex6) be.launchTiles(tvw.nTiles, ProdTileA<6>{mv, par, sv, rv, av, pv, tvw});
-        else be.launchTiles(tvw.nTiles, ProdTileA<0>{mv, par, sv, rv, av, pv, tvw});
+        withNF([&](auto nf) { be.launchTiles(tvw.nTiles, ProdTileA<nf>{mv, par, sv, rv, av, pv, tvw}); });
     }
     void launchTileBC(const PsiView& pv, double* y)
     {
-        if (hex6)
-        {
-            switch (featureMask())
-            {
-            case 0: be.launchTiles(tvw.nTiles, ProdTileBC<6, 0>{mv, par, sv, rv, av, pv, y, tvw}); break;
-            case 1: be.launchTiles(tvw.nTiles, ProdTileBC<6, 1>{mv, par, sv, rv, av, pv, y, tvw}); break;
-            case 2: be.launchTiles(tvw.nTiles, ProdTileBC<6, 2>{mv, par, sv, rv, av, pv, y, tvw}); break;
-            default: be.launchTiles(tvw.nTiles, ProdTileBC<6, 3>{mv, par, sv, rv, av, pv, y, tvw}); break;
-            }
-        }
-        else be.launchTiles(tvw.nTiles, ProdTileBC<0, 3>{mv, par, sv, rv, av, pv, y, tvw});
+        withNFF<3>([&](auto nf, auto ft) { be.launchTiles(tvw.nTiles, ProdTileBC<nf, ft>{mv, par, sv, rv, av, pv, y, tvw}); });
     }
 
     // initial states from the 0/ files (DASimpleFoam::initSolver createFieldsSimple.H role); phi = linear-interpolated U . Sf
@@ -1635,37 +1603,37 @@ struct Solver
         if (par.comp)
         {
             // DARhoSimpleFoam: closures + gradients, momentum/SA rows, energy row, pressure/flux rows (comp_kernels.hpp)
-            DAB_LAUNCH_NF(hm.nCtot, cFwdA, mv, par, sv, rv); // closures of the ghost cells come from their exchanged states
+            launchNF<cFwdA>(hm.nCtot, mv, par, sv, rv); // closures of the ghost cells come from their exchanged states
             if (exchange && ghosted())
             {
                 std::vector<HaloItem> it{{rv.gU, 9, 1, nT}, {rv.gP, 3, 1, nT}, {rv.gHe, 3, 1, nT}};
                 if (par.turb) it.push_back({rv.gNt, 3, 1, nT});
                 halo.exchangeCells(it);
             }
-            DAB_LAUNCH_NF(hm.nC, cFwdB, mv, par, sv, rv, isPC, Rdev);
-            DAB_LAUNCH_NF(hm.nC, cFwdE, mv, par, sv, rv, isPC, Rdev);
+            launchNF<cFwdB>(hm.nC, mv, par, sv, rv, isPC, Rdev);
+            launchNF<cFwdE>(hm.nC, mv, par, sv, rv, isPC, Rdev);
             if (exchange && ghosted()) halo.exchangeCells({{rv.rAU, 1, 1, nT}, {rv.HbyA, 3, 1, nT}, {rv.flag, 1, 1, nT}});
             if (isPC && par.transonic)
             {
                 Params pq = par; // div(pc) scheme and transonicPCOption for the preconditioner residual
                 pq.divPhidP = DIV_UPWIND;
                 pq.transonic = transonicPCOption == 1 ? 2 : (transonicPCOption == 2 ? 3 : 1);
-                DAB_LAUNCH_NF(hm.nC, cFwdC, mv, pq, sv, rv, Rdev);
+                launchNF<cFwdC>(hm.nC, mv, pq, sv, rv, Rdev);
             }
             else
-                DAB_LAUNCH_NF(hm.nC, cFwdC, mv, par, sv, rv, Rdev);
+                launchNF<cFwdC>(hm.nC, mv, par, sv, rv, Rdev);
             return;
         }
-        DAB_LAUNCH_NF(hm.nCtot, FwdA, mv, par, sv, rv);
+        launchNF<FwdA>(hm.nCtot, mv, par, sv, rv);
         if (exchange && ghosted())
         {
             std::vector<HaloItem> it{{rv.gU, 9, 1, nT}, {rv.gP, 3, 1, nT}};
             if (par.turb) it.push_back({rv.gNt, 3, 1, nT});
             halo.exchangeCells(it);
         }
-        DAB_LAUNCH_NFF(hm.nC, FwdB, mv, par, sv, rv, isPC, Rdev);
+        launchNFF<FwdB>(hm.nC, mv, par, sv, rv, isPC, Rdev);
         if (exchange && ghosted()) halo.exchangeCells({{rv.rAU, 1, 1, nT}, {rv.HbyA, 3, 1, nT}, {rv.flag, 1, 1, nT}});
-        DAB_LAUNCH_NF(hm.nC, FwdC, mv, par, sv, rv, Rdev);
+        launchNF<FwdC>(hm.nC, mv, par, sv, rv, Rdev);
     }
 
     void ensureRecorded()
@@ -1682,23 +1650,18 @@ struct Solver
         be.d2h(R, dR.p, (size_t)nDof() * sizeof(double));
     }
 
-    // y = diag(n) (dR/dW)^T x on device vectors (external layout)
-    void launchRevA(const PsiView& pv) { DAB_LAUNCH_NF(hm.nC, RevA, mv, par, sv, rv, av, pv); }
-
-    PsiView psiView(const double* x)
+    // psi's blocks in the state order U, p, [T], [nuTilda], phi.  On a ghosted mesh p, T, nuTilda and phi are copied into ghosted
+    // buffers and exchanged: awaited when `wait`, else only started (halo.finish() before the first reader)
+    PsiView psiView(const double* x, bool wait)
     {
         const size_t nC = hm.nC;
         PsiView v;
         v.U = x;
-        v.T = nullptr;
-        if (!ghosted())
-        {
-            v.p = x + 3 * nC;
-            v.T = par.comp ? x + 4 * nC : nullptr;
-            v.nt = x + (par.comp ? 5 : 4) * nC;
-            v.phi = x + (size_t)nCellStates() * nC;
-            return v;
-        }
+        v.p = x + 3 * nC;
+        v.T = par.comp ? x + 4 * nC : nullptr;
+        v.nt = x + (par.comp ? 5 : 4) * nC;
+        v.phi = x + (size_t)nCellStates() * nC;
+        if (!ghosted()) return v;
         const int nT = hm.nCtot;
         if (psiP.n < (size_t)nT)
         {
@@ -1706,116 +1669,108 @@ struct Solver
             psiN.alloc(be, nT);
             psiPhi.alloc(be, hm.nF);
         }
-        be.d2d(psiP.p, x + 3 * nC, nC * sizeof(double));
+        be.d2d(psiP.p, v.p, nC * sizeof(double));
         std::vector<HaloItem> it{{psiP.p, 1, 1, nT}};
         if (par.comp)
         {
             if (psiT.n < (size_t)nT) psiT.alloc(be, nT);
-            be.d2d(psiT.p, x + 4 * nC, nC * sizeof(double));
+            be.d2d(psiT.p, v.T, nC * sizeof(double));
             it.push_back({psiT.p, 1, 1, nT});
             v.T = psiT.p;
         }
         if (par.turb)
         {
-            be.d2d(psiN.p, x + (par.comp ? 5 : 4) * nC, nC * sizeof(double));
+            be.d2d(psiN.p, v.nt, nC * sizeof(double));
             it.push_back({psiN.p, 1, 1, nT});
         }
-        be.d2d(psiPhi.p, x + (size_t)nCellStates() * nC, (size_t)hm.nF * sizeof(double));
-        halo.exchangeCells(it);
-        halo.exchangeFaces({{psiPhi.p, 1, 1, hm.nF}});
+        be.d2d(psiPhi.p, v.phi, (size_t)hm.nF * sizeof(double));
+        if (wait)
+        {
+            halo.exchangeCells(it);
+            halo.exchangeFaces({{psiPhi.p, 1, 1, hm.nF}});
+        }
+        else
+        {
+            halo.start(halo.cells, it);
+            halo.start(halo.faces, {{psiPhi.p, 1, 1, hm.nF}});
+        }
         v.p = psiP.p;
         v.nt = psiN.p;
         v.phi = psiPhi.p;
         return v;
     }
 
+    // the ghost values a reverse stage leaves for the next: those of stage 0 for stage 1, those of stage 1 (and cRevE) for RevC / cRevC
+    std::vector<HaloItem> revGhosts(int s) const
+    {
+        const int nT = hm.nCtot;
+        if (s == 0) return {{av.mt, 3, 1, nT}, {av.Dn, 1, 1, nT}, {av.gPb, 3, 1, nT}};
+        std::vector<HaloItem> it{{av.gUb, 9, 1, nT}};
+        if (par.comp) it.push_back({av.gHeb, 3, 1, nT});
+        if (par.turb) it.push_back({av.gNtb, 3, 1, nT});
+        return it;
+    }
+
+    // stage s (0-2) of the reverse sweep; dab_bench_device selector 2 + s times it alone
+    //   incompressible: RevA, RevB, RevC over all owned cells with their L2 prefetch plans, or over the cell range *r
+    //   compressible (comp_rev_kernels.hpp): cRevA, cRevB, cRevE + cRevC; `exchange`: revGhosts(1) between cRevE and cRevC (blocking)
+    //   tile product: the RevA tile, the fused RevB + RevC tile, nothing
+    void revStage(int s, const PsiView& pv, double* y, const Cells* r = nullptr, bool exchange = false)
+    {
+        const int nC = hm.nC;
+        if (par.comp)
+        {
+            if (s == 0) launchNF<cRevA>(nC, mv, par, sv, rv, av, pv);
+            else if (s == 1) launchNF<cRevB>(nC, mv, par, sv, rv, av, pv, y);
+            else
+            {
+                launchNF<cRevE>(nC, mv, par, sv, rv, av, pv, y);
+                if (exchange) halo.exchangeCells(revGhosts(1));
+                launchNF<cRevC>(nC, mv, par, sv, rv, av, y);
+            }
+            return;
+        }
+        if (tileProduct())
+        {
+            if (s == 0) launchTileA(pv);
+            else if (s == 1) launchTileBC(pv, y);
+            return;
+        }
+        auto at = [&](const PfPlan& pl) { return r ? *r : Cells{nC, -1, pl}; };
+        if (s == 0) launchNF<RevA>(at(pfRevA(pv)), mv, par, sv, rv, av, pv);
+        else if (s == 1) launchNFF<RevB>(at(pfRevB(pv)), mv, par, sv, rv, av, pv, y);
+        else launchNF<RevC>(at(pfRevC()), mv, par, sv, rv, av, y, 0);
+    }
+
+    // y = diag(n) (dR/dW)^T x on device vectors (external layout)
     void matVecDev(const double* x, double* y)
     {
         ensureRecorded();
-        if (par.comp)
+        if (par.comp || !ghosted())
         {
-            // DARhoSimpleFoam reverse sweep (comp_rev_kernels.hpp), one GPU
-            const PsiView pv = psiView(x);
-            const int nTc = hm.nCtot;
-            DAB_LAUNCH_NF(hm.nC, cRevA, mv, par, sv, rv, av, pv);
-            if (ghosted()) halo.exchangeCells({{av.mt, 3, 1, nTc}, {av.Dn, 1, 1, nTc}, {av.gPb, 3, 1, nTc}});
-            DAB_LAUNCH_NF(hm.nC, cRevB, mv, par, sv, rv, av, pv, y);
-            DAB_LAUNCH_NF(hm.nC, cRevE, mv, par, sv, rv, av, pv, y);
-            if (ghosted())
-            {
-                std::vector<HaloItem> it{{av.gUb, 9, 1, nTc}, {av.gHeb, 3, 1, nTc}};
-                if (par.turb) it.push_back({av.gNtb, 3, 1, nTc});
-                halo.exchangeCells(it);
-            }
-            DAB_LAUNCH_NF(hm.nC, cRevC, mv, par, sv, rv, av, y);
-            return;
-        }
-        const int nT = hm.nCtot;
-        if (!ghosted())
-        {
-            const PsiView pv = psiView(x);
-            if (tileProduct())
-            {
-                launchTileA(pv);
-                launchTileBC(pv, y);
-                return;
-            }
-            DAB_LAUNCH_NF_PF(pfRevA(pv), hm.nC, RevA, mv, par, sv, rv, av, pv);
-            DAB_LAUNCH_NFF_PF(pfRevB(pv), hm.nC, RevB, mv, par, sv, rv, av, pv, y);
-            DAB_LAUNCH_NF_PF(pfRevC(), hm.nC, RevC, mv, par, sv, rv, av, y, 0);
+            // one rank without ghosts, or the compressible sweep with blocking exchanges
+            const PsiView pv = psiView(x, true);
+            revStage(0, pv, y);
+            if (ghosted()) halo.exchangeCells(revGhosts(0));
+            revStage(1, pv, y);
+            revStage(2, pv, y, nullptr, ghosted());
             return;
         }
         // several ranks: every ghost exchange runs on the communication stream while the interior cells (no neighbour on
         // another rank) of the next stage are processed; the cut-adjacent cells follow once the ghosts have arrived
-        const int nI = hm.nInterior < 0 ? hm.nC : hm.nInterior, nB = hm.nC - nI;
-        const PsiView pv = psiViewStart(x);
-        DAB_LAUNCH_NF_R(0, nI, RevA, mv, par, sv, rv, av, pv);
-        halo.finish();
-        DAB_LAUNCH_NF_R(nI, nB, RevA, mv, par, sv, rv, av, pv);
-        halo.start(halo.cells, {{av.mt, 3, 1, nT}, {av.Dn, 1, 1, nT}, {av.gPb, 3, 1, nT}});
-        DAB_LAUNCH_NFF_R(0, nI, RevB, mv, par, sv, rv, av, pv, y);
-        halo.finish();
-        DAB_LAUNCH_NFF_R(nI, nB, RevB, mv, par, sv, rv, av, pv, y);
+        const int nI = hm.nInterior < 0 ? hm.nC : hm.nInterior;
+        const Cells interior{nI, 0}, cut{hm.nC - nI, nI};
+        const PsiView pv = psiView(x, false);
+        for (int s = 0; s < 3; s++)
         {
-            std::vector<HaloItem> it{{av.gUb, 9, 1, nT}};
-            if (par.turb) it.push_back({av.gNtb, 3, 1, nT});
-            halo.start(halo.cells, it);
+            if (s > 0) halo.start(halo.cells, revGhosts(s - 1));
+            revStage(s, pv, y, &interior);
+            halo.finish();
+            revStage(s, pv, y, &cut);
         }
-        DAB_LAUNCH_NF_R(0, nI, RevC, mv, par, sv, rv, av, y, 0);
-        halo.finish();
-        DAB_LAUNCH_NF_R(nI, nB, RevC, mv, par, sv, rv, av, y, 0);
     }
 
-    // ghost values of the input vector, exchange started but not awaited (halo.finish() before the first reader)
-    PsiView psiViewStart(const double* x)
-    {
-        const size_t nC = hm.nC;
-        const int nT = hm.nCtot;
-        if (psiP.n < (size_t)nT)
-        {
-            psiP.alloc(be, nT);
-            psiN.alloc(be, nT);
-            psiPhi.alloc(be, hm.nF);
-        }
-        PsiView v;
-        v.U = x;
-        be.d2d(psiP.p, x + 3 * nC, nC * sizeof(double));
-        std::vector<HaloItem> it{{psiP.p, 1, 1, nT}};
-        if (par.turb)
-        {
-            be.d2d(psiN.p, x + 4 * nC, nC * sizeof(double));
-            it.push_back({psiN.p, 1, 1, nT});
-        }
-        be.d2d(psiPhi.p, x + (par.turb ? 5 : 4) * nC, (size_t)hm.nF * sizeof(double));
-        halo.start(halo.cells, it);
-        halo.start(halo.faces, {{psiPhi.p, 1, 1, hm.nF}});
-        v.p = psiP.p;
-        v.nt = psiN.p;
-        v.phi = psiPhi.p;
-        return v;
-    }
-
-    // one reverse kernel alone on the bench vectors (dab_bench_device selectors 2-4).  On several ranks the kernel runs over all owned
+    // one reverse stage alone on the bench vectors (dab_bench_device selectors 2-4).  On a ghosted mesh the stage runs over all owned
     // cells on the ghost values the last full product left behind: no copy, no exchange inside the timed launches
     void benchKernel(int which)
     {
@@ -1825,36 +1780,8 @@ struct Solver
             pv.U = dX.p; pv.p = psiP.p; pv.nt = psiN.p; pv.phi = psiPhi.p; pv.T = psiT.n ? psiT.p : nullptr;
         }
         else
-            pv = psiView(dX.p);
-        if (par.comp)
-        {
-            // DARhoSimpleFoam: 0 cRevA, 1 cRevB, 2 cRevE + cRevC
-            if (which == 0) DAB_LAUNCH_NF(hm.nC, cRevA, mv, par, sv, rv, av, pv);
-            else if (which == 1) DAB_LAUNCH_NF(hm.nC, cRevB, mv, par, sv, rv, av, pv, dY2.p);
-            else
-            {
-                DAB_LAUNCH_NF(hm.nC, cRevE, mv, par, sv, rv, av, pv, dY2.p);
-                DAB_LAUNCH_NF(hm.nC, cRevC, mv, par, sv, rv, av, dY2.p);
-            }
-            return;
-        }
-        if (tileProduct())
-        {
-            // tile kernels: 0 = RevA tile, 1 = fused RevB+RevC tile (there is no separate RevC)
-            if (which == 0) launchTileA(pv);
-            else if (which == 1) launchTileBC(pv, dY2.p);
-            return;
-        }
-        if (ghosted())
-        {
-            if (which == 0) launchRevA(pv);
-            else if (which == 1) DAB_LAUNCH_NFF(hm.nC, RevB, mv, par, sv, rv, av, pv, dY2.p);
-            else DAB_LAUNCH_NF(hm.nC, RevC, mv, par, sv, rv, av, dY2.p, 0);
-            return;
-        }
-        if (which == 0) DAB_LAUNCH_NF_PF(pfRevA(pv), hm.nC, RevA, mv, par, sv, rv, av, pv);
-        else if (which == 1) DAB_LAUNCH_NFF_PF(pfRevB(pv), hm.nC, RevB, mv, par, sv, rv, av, pv, dY2.p);
-        else DAB_LAUNCH_NF_PF(pfRevC(), hm.nC, RevC, mv, par, sv, rv, av, dY2.p, 0);
+            pv = psiView(dX.p, true);
+        revStage(which, pv, dY2.p);
     }
 
     void matVec(const double* x, double* y)
@@ -2271,9 +2198,9 @@ struct Solver
                 be.zero(av.gPb, (size_t)3 * hm.nCtot * sizeof(double));
                 be.zero(av.gNtb, (size_t)3 * hm.nCtot * sizeof(double));
                 be.zero(av.gHeb, (size_t)3 * hm.nCtot * sizeof(double));
-                DAB_LAUNCH_NF(hm.nC, cForceRevA, mv, par, sv, rv, av, specs[g], seed);
+                launchNF<cForceRevA>(hm.nC, mv, par, sv, rv, av, specs[g], seed);
                 if (ghosted()) halo.exchangeCells({{av.gUb, 9, 1, hm.nCtot}});
-                DAB_LAUNCH_NF(hm.nC, cRevC, mv, par, sv, rv, av, dY2.p);
+                launchNF<cRevC>(hm.nC, mv, par, sv, rv, av, dY2.p);
                 be.zero(dY2.p + (size_t)nCellStates() * hm.nC, (size_t)hm.nF * sizeof(double)); // no face-flux dependence
                 if (g == 0)
                     be.d2h(out, dY2.p, (size_t)nDof() * sizeof(double));
@@ -2290,13 +2217,13 @@ struct Solver
         be.zero(av.gUb, (size_t)9 * hm.nCtot * sizeof(double));
         be.zero(av.gPb, (size_t)3 * hm.nCtot * sizeof(double));
         be.zero(av.gNtb, (size_t)3 * hm.nCtot * sizeof(double));
-        DAB_LAUNCH_NF(hm.nC, ForceRevA, mv, par, sv, rv, av, specs[0], seed);
+        launchNF<ForceRevA>(hm.nC, mv, par, sv, rv, av, specs[0], seed);
         if (ghosted())
         {
             std::vector<HaloItem> it{{av.gUb, 9, 1, hm.nCtot}};
             halo.exchangeCells(it);
         }
-        DAB_LAUNCH_NF(hm.nC, RevC, mv, par, sv, rv, av, dY2.p, 1);
+        launchNF<RevC>(hm.nC, mv, par, sv, rv, av, dY2.p, 1);
         be.d2h(out, dY2.p, (size_t)nDof() * sizeof(double));
     }
 
